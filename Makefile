@@ -1,6 +1,6 @@
-# In-tree build of the C-ABI library (sm_100a only) and the CPU oracle.
+# In-tree build of the C-ABI library (sm_90a only) and the CPU oracle.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr -Iinclude
 CSRC := $(wildcard visionllm_b200/csrc/*.cu)
 OBJ := $(patsubst visionllm_b200/csrc/%.cu,build/%.o,$(CSRC))

@@ -1,11 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- the driver's measurement contract for the VisionLLMv2 forward hot path.
+"""bench.py -- throughput of the VisionLLMv2 forward hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 One JSON line on rank 0.  See DESIGN.md "Measurement" for what each field means.
 Workloads live in bench_workloads.py; the default is the most complete
-native path available (see DEFAULT_WORKLOAD there).
+native path available (see DEFAULT_WORKLOAD there).  Nothing is written next to
+the sources (no bytecode either), so the tree may be read-only; --dump-outputs
+writes what the last timed step computed to DIR, for output-for-output
+comparison of two builds (inputs and weights are seeded: same arguments, same
+inputs).
 """
 import argparse
 import json
@@ -15,13 +19,14 @@ import sys
 import threading
 import time
 
+sys.dont_write_bytecode = True
 ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -103,6 +108,9 @@ def main():
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
     ap.add_argument("--workload", default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB in all; "
+                         "larger arrays as a fixed seeded sample of their elements)")
     ap.add_argument("--cuprof", action="store_true",
                     help="wrap ONE extra device step in cudaProfilerStart/Stop (ncu --profile-from-start off)")
     args = ap.parse_args()
@@ -115,6 +123,8 @@ def main():
     name = args.workload or benchlib.DEFAULT_WORKLOAD
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs stores the outputs of the native timed path; it has no meaning with --impl reference")
         # The reference's CPU implementation of the path, on the host cores; rank 0 only.
         if rank != 0:
             return
@@ -164,6 +174,8 @@ def main():
         sampler.start()
     ms_dev, launches = timed(wl.step_device, args.steps, args.warmup)
     trace(f"device-resident steps timed: {ms_dev / args.steps:.2f} ms/step")
+    if args.dump_outputs and rank == 0:
+        benchlib.dump_outputs(wl.out, args.dump_outputs)
     if args.cuprof:
         torch.cuda.synchronize()
         torch.cuda.profiler.start()
@@ -196,8 +208,10 @@ def main():
         "e2e": {"value": units / (ms_e2e / args.steps / 1e3), "unit": wl.unit,
                 "h2d_bytes_per_step": wl.h2d_bytes, "d2h_bytes_per_step": wl.d2h_bytes,
                 "ms_per_step": ms_e2e / args.steps},
-        "gpu_launches": launches, "clocks": clocks, "roofline": roof,
+        "gpu_launches": launches, "gpu": benchlib.gpu_identity(local_rank), "clocks": clocks, "roofline": roof,
+        "max_memory_allocated_gb": torch.cuda.max_memory_allocated() / 2 ** 30,
     }
+    line["config"]["h100_80gb_peak_memory_gb"] = benchlib.H100_80GB_PEAK_GB.get(name)
     line.update(wl.extra())
     if tp_obj is not None:
         line["tp"] = tp_obj

@@ -1,4 +1,4 @@
-/* libvllm_b200.so -- C-ABI of the B200-native VisionLLMv2 forward hot path.
+/* libvllm_b200.so -- C-ABI of the H100-native (sm_90a) VisionLLMv2 forward hot path.
  *
  * Plain pointers and sizes only (no torch types).  All pointers are DEVICE
  * pointers unless the parameter name says `host`.  Every function is
@@ -12,7 +12,7 @@
  * caller silently falls back to grid_sample (grounding_dino/
  * modeling_ov_grounding_dino_mask_dn.py:777-779); this boundary reports them.
  *
- * Paths below are relative to /root/reference/VisionLLMv2/.
+ * Paths below are relative to the VisionLLMv2/ directory of the reference project.
  */
 #ifndef VLLM_B200_H
 #define VLLM_B200_H
@@ -27,7 +27,7 @@ extern "C" {
 #define VLLM_EUNSUPPORTED (-2) /* shape outside what the kernels implement */
 #define VLLM_EALIGN (-3)       /* pointer alignment the vector path needs is missing */
 
-/* Library identity / build info: "vllm_b200 <git-less version> sm_100a". */
+/* Library identity / build info: "vllm_b200 <git-less version> sm_90a". */
 const char* vllm_version(void);
 
 /* ---- Multi-scale deformable attention --------------------------------------
@@ -102,7 +102,7 @@ int vllm_msda_backward_f64(const double* value, const int64_t* spatial_shapes, c
 int vllm_msda_sample_indices_f32(const int64_t* spatial_shapes, const float* sampling_loc, int32_t* out_hwm,
                                  long long n_samples, int num_levels, int num_point, void* stream);
 /* Tuning knob for bench sweeps (process-global, not part of the drop-in API): 0 default; 1-4 tile shapes of the fp32
- * warp-gather kernel; 16 = experimental FHFMA.BF16 form of vllm_msda_forward_pairs (bf16 corner weights). */
+ * warp-gather kernel. */
 int vllm_msda_set_variant(int variant);
 /* Encoder shape (num_query == spatial_size, host_shapes_hint given, <= 4 levels, channels == 32): vllm_msda_forward_f32
  * (non-strict) and vllm_msda_forward_bf16v run the TMA-staged window kernel (csrc/msda_win.cu): one CTA per (image
@@ -154,7 +154,7 @@ int vllm_dcnv3_backward_f32(const float* input, const float* offset, const float
                             int stride_h, int stride_w, int pad_h, int pad_w, int dilation_h, int dilation_w,
                             float offset_scale, void* stream);
 
-/* ---- bf16 tensor-core GEMM with fused epilogue (tcgen05 / TMEM / TMA) ----------
+/* ---- bf16 tensor-core GEMM with fused epilogue (wgmma / TMA / mbarrier) ----------
  * C[M, n_out] = epi(A[M,K] . B[N,K]^T): every nn.Linear on the hot path
  * (internvit/modeling_intern_vit.py:112,124,172-173; modeling_visionllmv2.py:162-184;
  * HF LlamaDecoderLayer / internlm2/modeling_internlm2.py:235-360;
@@ -185,7 +185,8 @@ int vllm_gemm_bf16_rowmask(const void* A, int lda, const void* B, int ldb, void*
  * scatter GEMM alone.  A GEMM CTA owns its SM, so the link-bound exchange kernels of another stream (tensor-parallel
  * micro-batches, visionllm_b200/tp.py) overlap a GEMM only on SMs its grid leaves free. */
 int vllm_gemm_set_sm_limit(int all_gemms, int scatter_gemm);
-/* Tuning knob (process-global): 0 = auto (default), 1 = cta_group::1 tiles 128x256, 2 = CTA-pair tiles 256x256. */
+/* Tuning knob (process-global): 0 = auto (default: 128x128 tiles; the scatter GEMM always uses
+ * 128x256), 1 = 128x128 tiles, 2 = 128x256 tiles. */
 /* Stride-1 KxK convolution over a zero-padded channels-last map as ONE implicit GEMM (no im2col buffer): the 3x3
  * `output_convs` of the Grounding-DINO mask-feature FPN (modeling_ov_grounding_dino_mask_dn.py:2136-2146, :2476).
  * xpad: [pad_pixels, channels] bf16 = the padded images flattened (image rows of `padded_width` pixels, images back
@@ -243,8 +244,6 @@ int vllm_dcnv3_blend_bf16(const void* core, const void* xproj, const void* scale
  * [K*K][C] bf16, bias [C] bf16 or NULL, C % 8 == 0. */
 int vllm_dwconv_nhwc_bf16(const void* x, const void* weight_taps, const void* bias, void* y, int batch, int height,
                           int width, int channels, int kernel, void* stream);
-/* Tuning knob (process-global): 0 = default depthwise kernel, 1 = experimental FHFMA.BF16 variant (same arithmetic). */
-int vllm_dwconv_set_variant(int variant);
 /* GroupNorm over channels-last rows x[batch, hw, channels] (bf16, fp32 statistics, optional fused ReLU): the
  * nn.GroupNorm(32, d_model) after each Grounding-DINO input projection
  * (grounding_dino/modeling_ov_grounding_dino_mask_dn.py:2085-2110, :2393-2405) and the detectron2
@@ -321,8 +320,8 @@ int vllm_attention_bf16_tiles(const void* q, const void* k, const void* v, void*
                               long long o_token_pitch, const int* seqlens, const unsigned char* key_mask,
                               const unsigned char* attn_mask, float scale, const int* tile_counts,
                               const int* tile_lists, void* stream);
-/* Tuning knob (process-global), head_dim 128 without masks: 0 = tcgen05/TMEM kernel, schedule "tc2" (default),
- * 2 = tcgen05/TMEM ping-pong schedule, 1 = warp-MMA kernel always. */
+/* Tuning knob (process-global), head_dim 128 / 256 without attn_mask / attn_bias: 0 = wgmma kernel (default),
+ * 1 = warp-MMA kernel always. */
 int vllm_attention_set_variant(int variant);
 
 /* ---- tensor-parallel LLM decoder over peer memory (BASELINE cfg 5, SURVEY 8e) -------
@@ -382,9 +381,9 @@ int vllm_mask_postprocess_f32(const float* masks, const int64_t* box_idx, int nu
                               int crop_h, int crop_w, int out_h, int out_w, unsigned char* out, void* stream);
 
 /* ---- backward GEMMs (training-side path of BASELINE cfg 5) ----------------------------------------------------
- * C[M, N] = sum_k A(m, k) * B(n, k), bf16 in, fp32 accumulate, bf16 or fp32 out, same tcgen05 kernel as vllm_gemm_bf16.
+ * C[M, N] = sum_k A(m, k) * B(n, k), bf16 in, fp32 accumulate, bf16 or fp32 out, same wgmma kernel as vllm_gemm_bf16.
  * Each operand is either K-major ([M|N rows, K cols], pitch lda / ldb) or MN-major ([K rows, M|N cols]); MN-major tiles
- * are TMA-loaded as 64 x 64 boxes and fed to tcgen05.mma through MN-major shared-memory descriptors, so the backward
+ * are TMA-loaded as 64 x 64 boxes and fed to wgmma through MN-major shared-memory descriptors, so the backward
  * of y = x W^T (the reference's nn.Linear autograd, torch.nn.functional.linear) needs no transposed copies:
  *   dgrad  dx = dy . W      : A = dy [T, out] K-major,  B = W [out, in]  MN-major,  M = T,   N = in, K = out
  *   wgrad  dW = dy^T . x    : A = dy [T, out] MN-major, B = x [T, in]    MN-major,  M = out, N = in, K = T     */
@@ -393,7 +392,8 @@ int vllm_gemm_bf16_tn(const void* A, int lda, int a_mn_major, const void* B, int
 
 /* n_batch independent products in one launch (block-diagonal batching): every operand and C are stacks of their
  * n_batch matrices along the row axis.  causal: 0 none; 1 skip output tiles strictly above the diagonal (S = Q K^T,
- * dP = dO V^T); 2 / 3 restrict the K range to where a causal P / dS is non-zero (dV = P^T dO, dK = dS^T Q / dQ = dS K).
+ * dP = dO V^T); 2 / 3 restrict the K range to where a causal P / dS is non-zero (dV = P^T dO, dK = dS^T Q / dQ = dS K;
+ * K is the sequence axis there: K == M is required).
  * M % 256 == 0 (and K % 64 == 0 with MN-major operands) so tiles never straddle two matrices. */
 int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc,
                            int n_batch, int M, int N, int K, int causal, int out_f32, void* stream);

@@ -1,6 +1,6 @@
 /* ORACLE -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * CPU restatement of the reference DCNv3 forward as its CUDA kernel defines it:
- *   /root/reference/VisionLLMv2/visionllmv2/model/ops_dcnv3/src/cuda/dcnv3_im2col_cuda.cuh
+ *   VisionLLMv2/visionllmv2/model/ops_dcnv3/src/cuda/dcnv3_im2col_cuda.cuh
  *     :32-80   bilinear corner gather; :216-277 im2col loop (taps kernel_w-major, pixel-unit offsets * offset_scale,
  *     range test, col += val * mask).
  * fp32, every product/sum individually rounded (-ffp-contract=off): the reference GPU build may contract some of

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -19,7 +19,7 @@ def golden_dir():
 
 def pytest_collection_modifyitems(config, items):
     """`gpu`-marked tests need a CUDA device AND the in-tree library: skip (not fail) them elsewhere, so that a plain
-    `pytest tests` on the build box is green; on a GPU box a missing library is still a hard error inside the tests."""
+    `pytest tests` on a machine without a GPU is green; on a GPU machine a missing library is still a hard error inside the tests."""
     try:
         import torch
         has_cuda = torch.cuda.is_available()
@@ -27,7 +27,7 @@ def pytest_collection_modifyitems(config, items):
         has_cuda = False
     if has_cuda:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (run under gpurun)")
+    skip = pytest.mark.skip(reason="needs a CUDA device")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -26,9 +26,9 @@ def ref_attn(q, k, v, causal, seqlens=None):
     return o
 
 
-@pytest.fixture(params=[0, 1, 2], ids=["tcgen05_tc2", "warp_mma", "tcgen05_pingpong"])
+@pytest.fixture(params=[0, 1], ids=["wgmma", "warp_mma"])
 def variant(request):
-    """Run every case on the tcgen05/TMEM kernel (head_dim 128) and on the warp-MMA kernel."""
+    """Run every case on the wgmma kernel (head_dim 128 / 256) and on the warp-MMA kernel."""
     from visionllm_b200 import _lib
     _lib.lib().vllm_attention_set_variant(request.param)
     yield request.param
@@ -51,6 +51,11 @@ def check(out, ref):
     (3, 130, 3, 128, True),
     (2, 257, 2, 128, False),      # one key past two KV tiles, one row past the first CTA
     (1, 3136, 2, 128, True),      # released-7B sequence length
+    (2, 900, 4, 256, False),      # GDINO bi-attention head width: two 128-column halves of O
+    (1, 200, 2, 256, True),
+    (2, 129, 3, 128, False),      # one row past the first query tile, one key past two KV tiles
+    (1, 4097, 1, 128, True),      # the K/V stage ring wraps many times
+    (4, 64, 6, 128, False),       # a single full KV tile
 ])
 def test_attention_packed_qkv(B, T, H, D, causal, variant):
     from visionllm_b200 import ops
@@ -61,10 +66,11 @@ def test_attention_packed_qkv(B, T, H, D, causal, variant):
     check(out, ref_attn(q, k, v, causal))
 
 
-def test_attention_gqa_and_seqlens_and_cross(variant):
+@pytest.mark.parametrize("Hkv", [2, 4])
+def test_attention_gqa_and_seqlens_and_cross(variant, Hkv):
     from visionllm_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(1)
-    B, Tq, Tk, H, Hkv, D = 3, 200, 333, 8, 2, 128
+    B, Tq, Tk, H, D = 3, 200, 333, 8, 128
     q = torch.randn(B, Tq, H, D, device="cuda", generator=g).bfloat16()
     k = torch.randn(B, Tk, Hkv, D, device="cuda", generator=g).bfloat16()
     v = torch.randn(B, Tk, Hkv, D, device="cuda", generator=g).bfloat16()
@@ -74,12 +80,13 @@ def test_attention_gqa_and_seqlens_and_cross(variant):
     check(ops.attention(q, k, v, seqlens=sl), ref_attn(q, k, v, False, sl))
 
 
-def test_attention_large_magnitude_is_stable(variant):
+@pytest.mark.parametrize("D", [128, 256])
+def test_attention_large_magnitude_is_stable(variant, D):
     from visionllm_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(2)
-    q = (torch.randn(1, 256, 2, 128, device="cuda", generator=g) * 8).bfloat16()
-    k = (torch.randn(1, 256, 2, 128, device="cuda", generator=g) * 8).bfloat16()
-    v = torch.randn(1, 256, 2, 128, device="cuda", generator=g).bfloat16()
+    q = (torch.randn(1, 256, 2, D, device="cuda", generator=g) * 8).bfloat16()
+    k = (torch.randn(1, 256, 2, D, device="cuda", generator=g) * 8).bfloat16()
+    v = torch.randn(1, 256, 2, D, device="cuda", generator=g).bfloat16()
     out = ops.attention(q, k, v)
     assert torch.isfinite(out.float()).all()
     check(out, ref_attn(q, k, v, False))
@@ -100,7 +107,7 @@ def test_attention_head_dim_256_and_key_mask():
     s = s.masked_fill(~km[:, None, None, :], float("-inf"))
     ref = (torch.softmax(s, -1) @ v.float().permute(0, 2, 1, 3)).permute(0, 2, 1, 3).reshape(B, Tq, H * D)
     check(out, ref)
-    # head_dim 128 with a key mask: tcgen05 kernel with the mask operand (r2)
+    # head_dim 128 with a key mask: the wgmma kernel with the mask operand
     q2, k2, v2 = q[..., :128].contiguous(), k[..., :128].contiguous(), v[..., :128].contiguous()
     out2 = ops.attention(q2, k2, v2, key_mask=km)
     s2 = (q2.float().permute(0, 2, 1, 3) @ k2.float().permute(0, 2, 3, 1)) * 128 ** -0.5
@@ -148,10 +155,10 @@ def test_attention_split_kv_few_queries_many_keys(D, H):
 
 @pytest.mark.parametrize("D", [128, 256])
 @pytest.mark.parametrize("Tq,Tk", [(300, 80), (80, 4352), (257, 640), (1500, 96)])
-def test_attention_tcgen05_key_mask_and_split_kv(D, Tq, Tk):
-    """r2: head_dim 256 and key-masked head_dim 128 calls run on the tcgen05 kernel (attention_tc2.cu<D, KM>): the
+def test_attention_wgmma_key_mask_and_split_kv(D, Tq, Tk):
+    """head_dim 256 and key-masked head_dim 128 calls run on the wgmma kernel (attention_wgmma.cu<D, KM>): the
     GDINO bi-attention's two shapes (many vision queries x 80 text keys; 80 text queries x thousands of vision keys,
-    split along the key axis) with arbitrary key masks -- 16-byte mask loads (Tk % 16 == 0), fully masked 64-key tiles,
+    split along the key axis) with arbitrary key masks -- fully masked 64-key tiles,
     a batch entry whose mask leaves a single key.  Checked against fp32 torch and against the warp-MMA kernel."""
     from visionllm_b200 import _lib, ops
     g = torch.Generator(device="cuda").manual_seed(D + Tq + Tk)

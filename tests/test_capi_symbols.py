@@ -34,7 +34,7 @@ def test_python_binding_covers_the_header():
 
 
 def test_version_string():
-    assert b"sm_100a" in _lib.lib().vllm_version()
+    assert b"sm_90a" in _lib.lib().vllm_version()
 
 
 def test_round2_entry_points_marshal_and_accept_empty_problems():

@@ -42,7 +42,7 @@ def stage_config():
 
 @pytest.fixture(scope="module", params=["hf_swin", "b200_swin"])
 def stage(golden_dir, request):
-    """Backbone either HF's SwinBackbone run by torch (how the reference builds it) or ours on the B200 kernels."""
+    """Backbone either HF's SwinBackbone run by torch (how the reference builds it) or ours on the H100 kernels."""
     from weights_util import key_shapes, seeded_state_dict
     from visionllm_b200.gdino_model import B200GroundingDinoForObjectDetection
     from visionllm_b200.swin import B200SwinBackbone

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM + fused epilogues and the row kernels, against a plain
+"""GPU parity of the wgmma GEMM + fused epilogues and the row kernels, against a plain
 PyTorch fp32 reference of the same op on the same bf16-rounded inputs.
 
 Tolerance (written here as the north-star asks): inputs are bf16 and accumulation is fp32
@@ -12,7 +12,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-# cta_group variants under test (bring-up: VLLM_TEST_GEMM_VARIANTS=1 isolates the single-CTA kernel)
+# tile-width variants under test (bring-up: VLLM_TEST_GEMM_VARIANTS=1 isolates the 128-column tile)
 VARIANTS = [int(v) for v in os.environ.get("VLLM_TEST_GEMM_VARIANTS", "1,2").split(",")]
 
 
@@ -188,7 +188,7 @@ def test_rope_matches_hf_formula():
 @pytest.mark.parametrize("T,out_f,in_f", [(512, 256, 384), (2048, 4096, 4096), (300, 1376, 4096), (1000, 520, 200)])
 def test_gemm_tn_dgrad_wgrad_match_torch(T, out_f, in_f, variant):
     """dx = dy . W and dW = dy^T . x through vllm_gemm_bf16_tn vs fp32 torch on the same bf16 inputs (one bf16 output
-    rounding + 1e-3 max|ref|), both CTA-group variants, ragged M / N / K tails."""
+    rounding + 1e-3 max|ref|), both tile widths, ragged M / N / K tails."""
     from visionllm_b200 import _lib, ops
     g = torch.Generator(device="cuda").manual_seed(T + out_f)
     dy = (torch.randn(T, out_f, device="cuda", generator=g) * 0.5).bfloat16()

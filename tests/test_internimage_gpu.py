@@ -122,24 +122,3 @@ def test_layernorm_residual_matches_fp32():
     y = ops.layernorm(x, w, b, 1e-6, residual=r)
     ref = r.float() + F.layer_norm(x.float(), (640,), w.float(), b.float(), 1e-6)
     assert ((y.float() - ref).abs() <= 2.0 ** -8 * ref.abs() + 2e-3).all()
-
-
-@pytest.mark.skipif(os.environ.get("VLLM_EXPERIMENTAL") != "1", reason="opt-in: experimental kernel variants not yet "
-                    "validated on hardware (set VLLM_EXPERIMENTAL=1)")
-def test_dwconv_fhfma_variant_is_bit_identical():
-    """vllm_dwconv_set_variant(1): FHFMA.BF16 (bf16 x bf16 products are exact in fp32) must reproduce the default
-    unpack + FFMA kernel bit for bit."""
-    from visionllm_b200 import _lib, ops
-    g = torch.Generator(device="cuda").manual_seed(1)
-    x = torch.randn(2, 33, 47, 320, device="cuda", generator=g).bfloat16()
-    try:
-        for k in (3, 5, 7):
-            wt = (torch.randn(k * k, 320, device="cuda", generator=g) / k).bfloat16()
-            b = torch.randn(320, device="cuda", generator=g).bfloat16()
-            _lib.lib().vllm_dwconv_set_variant(0)
-            y0 = ops.dwconv_nhwc(x, wt, b, k)
-            _lib.lib().vllm_dwconv_set_variant(1)
-            y1 = ops.dwconv_nhwc(x, wt, b, k)
-            assert torch.equal(y0, y1), k
-    finally:
-        _lib.lib().vllm_dwconv_set_variant(0)

@@ -1,4 +1,4 @@
-"""CPU: host logic of the B200 region encoder (visionllm_b200/region_encoder.py) against the reference's own
+"""CPU: host logic of the H100 region encoder (visionllm_b200/region_encoder.py) against the reference's own
 `RegionEncoder` run (tests/golden/mod_region_encoder.npz): parameter names, patchify-conv row order, the cumulative
 `masks_out` across feature levels, the three pooling modes ('grid_sample' with the reference's recorded point draw).
 Kernels are replaced IN THIS TEST ONLY by fp32 torch / the MSDA oracle."""

@@ -6,7 +6,7 @@
   pointer tables, receive slots, gather buffer, counters and epochs exactly as in the multi-process run -- compared
   with the unsharded `B200LlamaForCausalLM` and with HF `LlamaForCausalLM` (fp32 and bf16, the module tolerance rule of
   test_modules_gpu.py), twice in a row (epoch counters);
-* multi-process over CUDA IPC + NVLink when the box has >= 2 GPUs (skipped otherwise; `gpurun --gpus 2`).
+* multi-process over CUDA IPC + NVLink when the machine has >= 2 GPUs (skipped otherwise).
 """
 import os
 import socket
@@ -30,7 +30,7 @@ def _flag(comm, off):
     return int(raw[off:off + 4].view(torch.int32).item())
 
 
-@pytest.mark.parametrize("K", [128, 1024])          # cta_group::1 and CTA-pair GEMM variants
+@pytest.mark.parametrize("K", [128, 1024])          # short and long K
 def test_scatter_gemm_fills_owner_slots(K):
     from visionllm_b200 import tp
     W, M, H = 2, 512, 320                            # H % 256 != 0: ragged last column tile
@@ -226,7 +226,7 @@ dist.destroy_process_group()
 """
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_tp_two_processes_over_ipc(tmp_path):
     script = tmp_path / "tp_worker.py"
     script.write_text(_WORKER)

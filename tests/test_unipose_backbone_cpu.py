@@ -1,4 +1,4 @@
-"""CPU: host logic of UniPose's image backbone on the B200 modules (visionllm_b200/unipose_backbone.py: reference
+"""CPU: host logic of UniPose's image backbone on the H100 modules (visionllm_b200/unipose_backbone.py: reference
 parameter names, patch-embed / window / merge padding, shift masks, relative-position bias slabs, out-index norms, mask
 interpolation, sine position embedding) against the reference's own `Joiner(SwinTransformer, PositionEmbeddingSineHW)`
 (tests/golden/mod_unipose_backbone.npz from gen_golden_unipose_backbone.py).  Kernels replaced IN THIS TEST ONLY by the

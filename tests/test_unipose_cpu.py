@@ -1,4 +1,4 @@
-"""CPU: host logic of the B200 UniPose deformable layers (visionllm_b200/unipose.py) against the reference's own
+"""CPU: host logic of the H100 UniPose deformable layers (visionllm_b200/unipose.py) against the reference's own
 classes (tests/golden/mod_unipose_layers.npz from gen_golden_unipose.py): parameter names, `True = padding` mask
 conventions, sequence-first decoder tensors, nn.MultiheadAttention attn_mask / key_padding_mask semantics, 2-d and 4-d
 reference points.  Kernels replaced IN THIS TEST ONLY by the fp32 stand-ins of test_gdino_logic_cpu."""
@@ -47,7 +47,7 @@ def test_unipose_layers_logic_matches_reference(golden_dir, torch_kernels):  # n
 
 # ---- two-stage keypoint decoder (modeling_unipose.py:2869-3130) -------------------------------------------------------
 def build_decoder():
-    """The B200 decoder built exactly like tests/golden/gen_golden_unipose_decoder.py builds the reference's."""
+    """The H100 decoder built exactly like tests/golden/gen_golden_unipose_decoder.py builds the reference's."""
     import types
 
     import torch.nn as nn

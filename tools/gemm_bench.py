@@ -1,5 +1,6 @@
-"""GPU: TFLOP/s of the tcgen05 GEMM (both variants) at the hot-path shapes; torch.matmul (cuBLAS) beside it."""
-import json, os, sys
+"""GPU: TFLOP/s of the wgmma GEMM (both tile widths) at the hot-path shapes; torch.matmul (cuBLAS) beside it.
+Usage: python tools/gemm_bench.py [out.json]   (the card's name and power limit are recorded with the numbers)"""
+import json, os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from visionllm_b200 import ops, _lib
@@ -7,11 +8,12 @@ from visionllm_b200 import ops, _lib
 SHAPES = {"vit_qkv": (41000, 9600, 3200), "vit_proj": (41000, 3200, 3200), "vit_fc1": (41000, 12800, 3200),
           "vit_fc2": (41000, 3200, 12800), "llm_qkv": (12288, 12288, 4096), "llm_gateup": (12288, 22016, 4096),
           "llm_down": (12288, 4096, 11008), "gdino_ffn1": (21760 * 8, 2048, 256), "sq8k": (8192, 8192, 8192)}
-res = {}
+res = {"gpu": subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True).stdout.strip()}
 
 
-def timeit(fn, iters=5):
-    for _ in range(2):
+def timeit(fn, iters=10):
+    for _ in range(3):
         fn()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -28,18 +30,18 @@ for name, (M, N, K) in SHAPES.items():
     out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
     fl = 2.0 * M * N * K
     r = {}
-    for v in (1, 2):
+    for v, nm in ((1, "tile128x128"), (2, "tile128x256")):
         _lib.lib().vllm_gemm_set_variant(v)
         try:
             ms = timeit(lambda: ops.linear(x, w, out=out))
-            r[f"cg{v}_tflops"] = fl / ms / 1e9
+            r[f"{nm}_tflops"] = fl / ms / 1e9
         except Exception as e:
-            r[f"cg{v}_error"] = str(e)
+            r[f"{nm}_error"] = str(e)
     _lib.lib().vllm_gemm_set_variant(0)
     ms = timeit(lambda: torch.matmul(x, w.T, out=out))
     r["cublas_tflops"] = fl / ms / 1e9
     res[name] = r
     print(name, r, flush=True)
     del x, w, out
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(res, open("gpurun_out/gemm_bench.json", "w"), indent=1)
+if len(sys.argv) > 1:
+    json.dump(res, open(sys.argv[1], "w"), indent=1)

@@ -1,4 +1,4 @@
-"""visionllm_b200 -- B200-native (sm_100a) forward hot path of VisionLLM v2.
+"""visionllm_b200 -- H100-native (sm_90a) forward hot path of VisionLLM v2.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed);
 compute is hand-written CUDA behind the C-ABI library ``lib/libvllm_b200.so``

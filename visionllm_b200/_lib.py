@@ -70,7 +70,6 @@ _SIGNATURES = {
     "vllm_layernorm_residual_bf16": (ci, [vp, cll, vp, vp, vp, cll, vp, cll, cll, ci, cf, vp]),
     "vllm_dcnv3_prep_f32": (ci, [vp, cll, vp, vp, vp, cll, ci, ci, vp]),
     "vllm_dcnv3_blend_bf16": (ci, [vp, vp, vp, vp, cll, ci, ci, vp]),
-    "vllm_dwconv_set_variant": (ci, [ci]),
     "vllm_dwconv_nhwc_bf16": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]),
     "vllm_rope_bf16": (ci, [vp, cll, vp, vp, cll, ci, ci, vp]),
     "vllm_groupnorm_workspace_bytes": (cll, [ci, ci]),

@@ -1,4 +1,4 @@
-"""B200-native CLIP vision tower (the released-7B preset's encoder, SURVEY 8a-a6): drop-in for HF
+"""H100-native CLIP vision tower (the released-7B preset's encoder, SURVEY 8a-a6): drop-in for HF
 ``CLIPVisionModel`` as the reference calls it (visionllmv2/model/modeling_visionllmv2.py:135,565-571:
 ``vis_encoder(x, output_hidden_states=True).hidden_states[-2][:, 1:]``).  The arithmetic lives in third-party
 transformers (pinned 4.34.0, not vendored); parity is checked against the installed ``CLIPVisionModel``.

@@ -5,12 +5,13 @@
 //   HF Llama FA2 / internlm2/modeling_internlm2.py:494-546 (causal, d=128, 32 heads, GQA for InternLM2)
 // and the naive paths (internvit/modeling_intern_vit.py:145-160; modeling_internlm2.py:362-411).
 //
-// Round-1 implementation: FlashAttention-2 dataflow on the legacy warp-level tensor path
+// This file: FlashAttention-2 dataflow on the warp-level tensor path
 // (ldmatrix + mma.sync.m16n8k16 bf16, fp32 accumulate) with online softmax in registers,
 // cp.async double-buffered K/V tiles in XOR-swizzled shared memory.  CTA = 64 query rows x one head
 // (4 warps x 16 rows), K/V tiles of 64 keys.  Scores never touch HBM: traffic = Q, K, V read once
-// per CTA wave + O written once.  The tcgen05/TMEM version (S and O accumulators in TMEM) is the
-// planned replacement; attention is ~5-6 % of the forward FLOPs (SURVEY.md 8a-a2/a10).
+// per CTA wave + O written once.  It serves head_dim 32 / 64, every attn_mask / attn_bias call and views TMA cannot
+// describe; head_dim 128 / 256 otherwise run on the wgmma kernel (attention_wgmma.cu).  Attention is ~5-6 % of the
+// forward FLOPs (SURVEY.md 8a-a2/a10).
 //
 // Layout: q/k/v are [batch, tokens, heads, D] views with arbitrary token/batch pitches (elements), so the
 // packed qkv GEMM output is consumed in place; o is [batch, tokens, heads*D].  seqlens (optional, int32
@@ -539,7 +540,7 @@ int launch(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long wo
   const int n_tiles = (a.Tk + BN - 1) / BN;
   if (workspace && !a.causal && !a.tile_counts && ctas < 2LL * vllm_num_sms() && n_tiles >= 16) {
     // pick the split count that minimises (waves of resident CTAs) x (key tiles per split): a count that spills a
-    // few CTAs into one more wave costs a whole extra pass (ncu: 640 CTAs on 296 slots = 2.16 waves ran as 3)
+    // few CTAs into one more wave costs a whole extra pass
     static int per_sm = 0;
     if (!per_sm) {
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, flash_fwd_kernel<D, BN>, NW * 32, SMEM) != cudaSuccess ||
@@ -571,42 +572,35 @@ int launch(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long wo
 
 }  // namespace
 
-int vllm_attention_tc_d128(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
-                           int kv_heads, long long q_bs, long long q_ts, long long k_bs, long long k_ts, long long v_bs,
-                           long long v_ts, long long o_bs, long long o_ts, const int* seqlens, int causal, float scale,
-                           cudaStream_t st);
-int vllm_attention_tc2_d128(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
-                            int kv_heads, long long q_bs, long long q_ts, long long k_bs, long long k_ts, long long v_bs,
-                            long long v_ts, long long o_bs, long long o_ts, const int* seqlens, int causal, float scale,
-                            cudaStream_t st);
-int vllm_attention_tc2(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
-                       int kv_heads, int head_dim, long long q_bs, long long q_ts, long long k_bs, long long k_ts,
-                       long long v_bs, long long v_ts, long long o_bs, long long o_ts, const int* seqlens,
-                       const unsigned char* key_mask, int causal, float scale, int n_splits, float* ws, cudaStream_t st);
+int vllm_attention_wgmma(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
+                         int kv_heads, int head_dim, long long q_bs, long long q_ts, long long k_bs, long long k_ts,
+                         long long v_bs, long long v_ts, long long o_bs, long long o_ts, const int* seqlens,
+                         const unsigned char* key_mask, int causal, float scale, int n_splits, float* ws, cudaStream_t st);
 
-// tcgen05 path for head_dim 256 and for key-masked head_dim 128 calls (r2): picks a split-KV count like launch<> below
+// wgmma path for head_dim 256 and for key-masked head_dim 128 calls: picks a split-KV count like launch<> above
 // when the query tiles alone cannot fill the SMs, then merges the partials with the same combine kernel.
 template <int D>
-static int launch_tc2_split(const AttnArgs& a, int batch, float scale, cudaStream_t st, void* workspace,
-                            long long workspace_bytes) {
+static int launch_wgmma_split(const AttnArgs& a, int batch, float scale, cudaStream_t st, void* workspace,
+                              long long workspace_bytes) {
   const int q_tiles = (a.Tq + 127) / 128;
   const long long ctas = (long long)q_tiles * a.heads * batch;
   const int n_tiles = (a.Tk + 63) / 64;
   long long best = 1;
   if (workspace && !a.causal && ctas < 2LL * vllm_num_sms() && n_tiles >= 16) {
-    const long long slots = (long long)vllm_num_sms() * (D == 128 ? 2 : 1);
+    const long long slots = vllm_num_sms();                               // one CTA per SM
     long long best_cost = (ctas + slots - 1) / slots * (n_tiles + 4);
     const long long max_s = n_tiles / 4 < 64 ? n_tiles / 4 : 64;
     for (long long sp = 2; sp <= max_s; ++sp) {
       if ((long long)batch * a.heads * sp * a.Tq * (D + 2) * 4 > workspace_bytes) break;
+      if ((sp - 1) * ((n_tiles + sp - 1) / sp) >= n_tiles) continue;      // the last split(s) would get no key tile at all
       const long long waves = (ctas * sp + slots - 1) / slots;
       const long long cost = waves * ((n_tiles + sp - 1) / sp + 4);       // +4 tiles: Q load, prologue, partial write-out
       if (cost < best_cost) { best_cost = cost; best = sp; }
     }
   }
-  const int rc = vllm_attention_tc2(a.q, a.k, a.v, a.o, batch, a.Tq, a.Tk, a.heads, a.kv_heads, D, a.q_bs, a.q_ts, a.k_bs,
-                                    a.k_ts, a.v_bs, a.v_ts, a.o_bs, a.o_ts, a.seqlens, a.key_mask, a.causal, scale, (int)best,
-                                    best > 1 ? (float*)workspace : nullptr, st);
+  const int rc = vllm_attention_wgmma(a.q, a.k, a.v, a.o, batch, a.Tq, a.Tk, a.heads, a.kv_heads, D, a.q_bs, a.q_ts, a.k_bs,
+                                      a.k_ts, a.v_bs, a.v_ts, a.o_bs, a.o_ts, a.seqlens, a.key_mask, a.causal, scale,
+                                      (int)best, best > 1 ? (float*)workspace : nullptr, st);
   if (rc != VLLM_OK || best == 1) return rc;
   const long long n_rows = (long long)batch * a.heads * a.Tq;
   splitkv_combine_kernel<D><<<(unsigned)((n_rows + 3) / 4), 128, 0, st>>>((const float*)workspace, a.o, a.o_bs, a.o_ts, a.Tq,
@@ -615,8 +609,7 @@ static int launch_tc2_split(const AttnArgs& a, int batch, float scale, cudaStrea
   return VLLM_OK;
 }
 
-// head_dim 128 without masks: 0 = tcgen05 "tc2" schedule (default: 1 Q tile/CTA, 2 CTAs/SM, double-buffered S),
-// 2 = tcgen05 ping-pong schedule (attention_tc.cu); 1 = always the warp-MMA kernel.
+// head_dim 128 / 256 without attn_mask / attn_bias: 0 = the wgmma kernel (attention_wgmma.cu), 1 = always the warp-MMA kernel.
 static int g_attn_variant = 0;
 extern "C" int vllm_attention_set_variant(int v) { g_attn_variant = v; return VLLM_OK; }
 
@@ -649,21 +642,15 @@ static int attention_impl(const void* q, const void* k, const void* v, void* o, 
   a.tile_counts = tile_counts; a.tile_lists = tile_lists; a.q_blocks = (Tq + 63) / 64; a.k_tiles = (Tk + 63) / 64;
   cudaStream_t st = (cudaStream_t)stream;
   if (head_dim == 128 && g_attn_variant == 0 && !key_mask && !attn_mask && !attn_bias) {
-    const int rc = vllm_attention_tc2_d128(q, k, v, o, batch, Tq, Tk, heads, kv_heads, q_batch_pitch, q_token_pitch,
-                                           k_batch_pitch, k_token_pitch, v_batch_pitch, v_token_pitch, o_batch_pitch,
-                                           o_token_pitch, seqlens, causal, scale, st);
-    if (rc != VLLM_EUNSUPPORTED) return rc;
+    const int rc = vllm_attention_wgmma(q, k, v, o, batch, Tq, Tk, heads, kv_heads, 128, q_batch_pitch, q_token_pitch,
+                                        k_batch_pitch, k_token_pitch, v_batch_pitch, v_token_pitch, o_batch_pitch,
+                                        o_token_pitch, seqlens, nullptr, causal, scale, 1, nullptr, st);
+    if (rc != VLLM_EUNSUPPORTED) return rc;   // views a TMA descriptor cannot express use the warp-MMA kernel
   }
   if ((head_dim == 256 || (head_dim == 128 && key_mask)) && g_attn_variant == 0 && !attn_mask && !attn_bias) {
-    const int rc = head_dim == 256 ? launch_tc2_split<256>(a, batch, scale, st, workspace, workspace_bytes)
-                                   : launch_tc2_split<128>(a, batch, scale, st, workspace, workspace_bytes);
+    const int rc = head_dim == 256 ? launch_wgmma_split<256>(a, batch, scale, st, workspace, workspace_bytes)
+                                   : launch_wgmma_split<128>(a, batch, scale, st, workspace, workspace_bytes);
     if (rc != VLLM_EUNSUPPORTED) return rc;
-  }
-  if (head_dim == 128 && g_attn_variant == 2 && !key_mask && !attn_mask && !attn_bias) {
-    const int rc = vllm_attention_tc_d128(q, k, v, o, batch, Tq, Tk, heads, kv_heads, q_batch_pitch, q_token_pitch,
-                                          k_batch_pitch, k_token_pitch, v_batch_pitch, v_token_pitch, o_batch_pitch,
-                                          o_token_pitch, seqlens, causal, scale, st);
-    if (rc != VLLM_EUNSUPPORTED) return rc;   // views a TMA descriptor cannot express use the warp-MMA kernel
   }
   // Swin windows: head_dim 32, one key tile, additive bias only -> one warp per (window, head) (variant 1 keeps the general kernel)
   if (head_dim == 32 && g_attn_variant != 1 && attn_bias && !key_mask && !attn_mask && !seqlens && !causal && Tq == Tk && Tq <= 64 &&

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels behind libvllm_b200.so.
+// Shared helpers for the sm_90a kernels behind libvllm_b200.so.
 // Everything here is device/host plumbing; no torch types anywhere in csrc/.
 #pragma once
 #include <cuda_runtime.h>
@@ -35,5 +35,13 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// Number of SMs of the current device (cached per process; B200 = 148).
+// Per-device one-time set-up (cudaFuncSetAttribute is a property of the function ON A DEVICE): the flag of the current
+// device in a caller-owned array, or nullptr when the device cannot be told (then the caller repeats the set-up).
+static inline bool* vllm_device_flag(bool (&flags)[64]) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
+  return &flags[dev];
+}
+
+// Number of SMs of the current device (cached per process; H100 SXM = 132).
 int vllm_num_sms();

@@ -1,4 +1,4 @@
-// DCNv3 forward (InternImage's core operator) for sm_100a.
+// DCNv3 forward (InternImage's core operator) for sm_90a.
 //
 // Replaces `dcnv3_forward` of the reference extension module `DCNv3`
 //   visionllmv2/model/ops_dcnv3/src/dcnv3.h:20-38 (pybind vision.cpp:14-17), host dcnv3_cuda.cu:21-85,

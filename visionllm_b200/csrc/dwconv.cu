@@ -86,96 +86,20 @@ dwconv_nhwc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __r
     if (w0 + p < W) *reinterpret_cast<uint4*>(yr + (size_t)(w0 + p) * C) = pack8(acc[p]);
 }
 
-// Experimental variant (vllm_dwconv_set_variant(1); default off, not validated on hardware yet): sm_100a's mixed-
-// precision FMA `fma.rn.f32.bf16` (SASS FHFMA.BF16 with .H0/.H1 operand selectors) multiplies two bf16 HALVES of 32-bit
-// registers and accumulates in fp32.  A bf16 x bf16 product is exact in fp32, so this is the same arithmetic as the
-// unpack + FFMA form above, without the unpack instructions (and with the input strip held as packed words).
-__device__ __forceinline__ void fma2_bf16(float& a0, float& a1, uint32_t x, uint32_t w) {
-  asm("{\n\t.reg .b16 xl, xh, wl, wh;\n\tmov.b32 {xl, xh}, %2;\n\tmov.b32 {wl, wh}, %3;\n\t"
-      "fma.rn.f32.bf16 %0, xl, wl, %0;\n\tfma.rn.f32.bf16 %1, xh, wh, %1;\n\t}"
-      : "+f"(a0), "+f"(a1) : "r"(x), "r"(w));
-}
-
-template <int K, int TW>
-__global__ void __launch_bounds__(128)
-dwconv_nhwc_fh_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ wt,
-                      const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ y, int N, int H, int W, int C,
-                      long long total) {
-  constexpr int R = K / 2;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int CV = C / 8, WT = (W + TW - 1) / TW;
-  const int cv = (int)(idx % CV);
-  long long t = idx / CV;
-  const int wt_i = (int)(t % WT); t /= WT;
-  const int h = (int)(t % H);
-  const int n = (int)(t / H);
-  const int w0 = wt_i * TW;
-  float acc[TW][8];
-  {
-    float b[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) b[j] = 0.f;
-    if (bias) unpack8(__ldg(reinterpret_cast<const uint4*>(bias) + cv), b);
-#pragma unroll
-    for (int p = 0; p < TW; ++p)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[p][j] = b[j];
-  }
-  const __nv_bfloat16* xn = x + (size_t)n * H * W * C + cv * 8;
-#pragma unroll 1
-  for (int dy = 0; dy < K; ++dy) {
-    const int hy = h + dy - R;
-    if (hy < 0 || hy >= H) continue;
-    uint4 in[TW + K - 1];
-#pragma unroll
-    for (int j = 0; j < TW + K - 1; ++j) {
-      const int wx = w0 + j - R;
-      in[j] = (wx >= 0 && wx < W) ? __ldg(reinterpret_cast<const uint4*>(xn + ((size_t)hy * W + wx) * C))
-                                  : make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int dx = 0; dx < K; ++dx) {
-      const uint4 wv = __ldg(reinterpret_cast<const uint4*>(wt + (size_t)(dy * K + dx) * C) + cv);
-#pragma unroll
-      for (int p = 0; p < TW; ++p) {
-        fma2_bf16(acc[p][0], acc[p][1], in[p + dx].x, wv.x);
-        fma2_bf16(acc[p][2], acc[p][3], in[p + dx].y, wv.y);
-        fma2_bf16(acc[p][4], acc[p][5], in[p + dx].z, wv.z);
-        fma2_bf16(acc[p][6], acc[p][7], in[p + dx].w, wv.w);
-      }
-    }
-  }
-  __nv_bfloat16* yr = y + (((size_t)n * H + h) * W) * C + cv * 8;
-#pragma unroll
-  for (int p = 0; p < TW; ++p)
-    if (w0 + p < W) *reinterpret_cast<uint4*>(yr + (size_t)(w0 + p) * C) = pack8(acc[p]);
-}
-
-int g_dwconv_variant = 0;
-
 template <int K>
 int launch_dw(const void* x, const void* wt, const void* bias, void* y, int N, int H, int W, int C, cudaStream_t st) {
   constexpr int TW = 4;
   const long long total = (long long)N * H * ((W + TW - 1) / TW) * (C / 8);
   const long long blocks = (total + 127) / 128;
   if (blocks > 2147483647LL) return VLLM_EUNSUPPORTED;
-  if (g_dwconv_variant == 1)
-    dwconv_nhwc_fh_kernel<K, TW><<<(unsigned)blocks, 128, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wt,
-                                                                   (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, N, H,
-                                                                   W, C, total);
-  else
-    dwconv_nhwc_kernel<K, TW><<<(unsigned)blocks, 128, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wt,
-                                                                (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, N, H, W,
-                                                                C, total);
+  dwconv_nhwc_kernel<K, TW><<<(unsigned)blocks, 128, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)wt,
+                                                              (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, N, H, W, C,
+                                                              total);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }
 
 }  // namespace
-
-/* Tuning knob (process-global): 0 = unpack + FFMA (default, validated), 1 = FHFMA.BF16 variant (experimental). */
-extern "C" int vllm_dwconv_set_variant(int v) { g_dwconv_variant = v == 1 ? 1 : 0; return VLLM_OK; }
 
 extern "C" int vllm_dwconv_nhwc_bf16(const void* x, const void* weight_taps, const void* bias, void* y, int batch,
                                      int height, int width, int channels, int kernel, void* stream) {

@@ -1,4 +1,4 @@
-// bf16 GEMM with fused epilogue on the sm_100a tensor cores (tcgen05 + TMEM + TMA).
+// bf16 GEMM with fused epilogue on the sm_90a tensor cores (wgmma + TMA + mbarrier).
 //
 //   C[M, N] = epilogue( A[M, K] . B[N, K]^T )      A, B bf16 K-major (B is an nn.Linear weight [out, in])
 //   epilogue: (+bias[N]) -> act -> (*colscale[N]) -> (+residual[M, N]) -> bf16 | fp32
@@ -11,24 +11,26 @@
 //   LLM        q/k/v/o, gate|up (SwiGLU), down(+residual)  (HF LlamaDecoderLayer; internlm2/modeling_internlm2.py:235-360)
 //   GDINO      value/offset/weight/output projections, FFN (ReLU)  (grounding_dino/...mask_dn.py:674-677,1116-1117)
 //
-// Structure (persistent, warp-specialised, one CTA or one CTA pair per SM):
-//   warp 0   TMA producer: A tile 128x64 and B tile (256|128)x64 bf16, 128B swizzle, STAGES-deep mbarrier ring
-//   warp 1   MMA issuer : one elected lane issues tcgen05.mma kind::f16, UMMA 128x256x16 (cta_group::1) or
-//            256x256x16 over a CTA pair (cta_group::2); fp32 accumulators in TMEM, 2 accumulator stages
-//            (2 x 256 columns) so the epilogue of tile i overlaps the main loop of tile i+1
-//   warp 2   TMEM allocator
-//   warps 4-11 epilogue (two warpgroups, one per 128-column half of the tile): tcgen05.ld 32 lanes x 32 columns ->
-//            registers -> fused math -> 16-byte global stores
+// Structure (persistent, warp-specialised, one CTA of three warpgroups per SM):
+//   warpgroup 0    producer: one elected lane of warp 0 issues the TMA loads, A tile 128x64 and B tile (256|128)x64
+//                  bf16, 128B swizzle, STAGES-deep mbarrier ring; the warpgroup hands its registers to the consumers
+//   warpgroups 1-2 consumers: warpgroup w owns rows 64(w-1)..64(w-1)+63 of the tile and issues wgmma m64n128k16
+//                  (one or two per k-step) straight from the swizzled stages; fp32 accumulators stay in registers
+//                  (64 x BN / 128 threads = 64 | 128 per thread).  One k-block of MMAs stays in flight while the next
+//                  stage is awaited; a stage goes back to the producer when the MMAs that read it have retired.
+//                  The fused epilogue runs on the accumulator fragments (a thread owns column pairs of two rows, so
+//                  the SwiGLU (gate, up) pair never leaves a thread); bf16 output is staged per warp in shared memory
+//                  and leaves as 128-byte row runs; the producer keeps prefetching the next tile's stages meanwhile.
 // Tiles are visited in groups of GROUP_M row-blocks so concurrently running CTAs share B (weights) in L2.
 #include "common.cuh"
 #include "tc_common.cuh"
 
 namespace {
 
-constexpr int BM = 128, BN = 256, BK = 64, ACC = 2, THREADS = 384, EPI_WARPS = 8;
+constexpr int BM = 128, BK = 64, THREADS = 384, CONSUMER_WARPS = 8, CONSUMER_THREADS = CONSUMER_WARPS * 32;
 constexpr int A_BYTES = BM * BK * 2;
-constexpr int EPI_PITCH = 128 + 16;                 // 64 bf16 columns + 16 B pad: conflict-free 16-byte accesses
-constexpr int EPI_STAGE_BYTES = 32 * EPI_PITCH;     // 32 rows per epilogue warp
+constexpr int EPI_PITCH = 128 + 16;                 // 64 bf16 columns + 16 B pad: conflict-free fragment writes and 16-byte reads
+constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH;      // a consumer warp's 16 rows of one 64-column chunk
 
 enum { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3, ACT_SWIGLU = 4, ACT_QUICKGELU = 5 };
 
@@ -38,21 +40,21 @@ struct GemmArgs {
   const __nv_bfloat16* bias; const __nv_bfloat16* colscale; const __nv_bfloat16* residual; int ldr;
   int act; int out_f32;
   const unsigned char* row_keep;   // optional [M]: rows with 0 are written as exact zeros (value.masked_fill of the MSDA module)
-  int tiles_m, tiles_n;  // tiles_m counts 128*CG-row blocks
+  int tiles_m, tiles_n;
   int group_m;           // row-blocks per rasterisation group (see pick_group_m)
   // Implicit convolution over a zero-padded channels-last image (vllm_conv_rows_bf16): the K axis is a_segs segments
   // of a_seg_kb k-blocks; segment s reads A rows shifted by s * a_seg_rows (one image row of the padded map), and a
   // row of the A tensor map spans kw consecutive pixels (row pitch = C elements, row length = kw*C: rows overlap).
   int a_seg_kb, a_seg_rows;
   // Fused reduce-scatter push (vllm_gemm_bf16_scatter, tensor-parallel o_proj): row block d = row / sc_rows of C goes
-  // to sc_dst[d] (a peer GPU's receive slot, row pitch ldc, local row = row - d * sc_rows); every epilogue warp bumps
+  // to sc_dst[d] (a peer GPU's receive slot, row pitch ldc, local row = row - d * sc_rows); every consumer warp bumps
   // sc_flag[d] once per tile after its stores (release at system scope).  sc_rows == 0: plain GEMM.
   int sc_rows;
   void* sc_dst[8];
   uint32_t* sc_flag[8];
   // MN-major operands (vllm_gemm_bf16_tn: the backward GEMMs -- dgrad reads the nn.Linear weight [N_red, K_out] as
   // B[j, k] = W[k, j], wgrad reads grad_output / activations [tokens, features] with the token axis as K): the operand
-  // is a row-major [K, MN] matrix; a 64-k x 64-mn TMA box is one 128B-swizzled MN-major UMMA atom row, chunks of 64 mn
+  // is a row-major [K, MN] matrix; a 64-k x 64-mn TMA box is one 128B-swizzled MN-major wgmma atom row, chunks of 64 mn
   // are 8 KB apart in the stage (LBO), 8 k-rows 1 KB apart (SBO), a k-step of 16 advances 2 KB.
   int a_mn, b_mn;
   // Block-diagonal batching (vllm_gemm_bf16_batched: the attention-backward GEMMs over all (batch, head) matrices of a
@@ -78,13 +80,12 @@ __device__ __forceinline__ TilePlan plan_tile(const GemmArgs& g, int m0, int n0,
   return p;
 }
 
-template <int CG> struct Cfg {
-  static constexpr int B_ROWS = BN / CG;               // B rows held by one CTA
-  static constexpr int B_BYTES = B_ROWS * BK * 2;
+template <int BN> struct Cfg {
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = CG == 1 ? 3 : 5;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 4 * BN * 4 /*bias, scale: double-buffered*/ +
-                              EPI_WARPS * EPI_STAGE_BYTES /*per-warp store staging*/;
+  static constexpr int STAGES = BN == 256 ? 4 : 6;     // 192 KB of operand stages either way
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2 * BN * 4 /*bias, scale*/ +
+                              CONSUMER_WARPS * EPI_WARP_BYTES /*per-warp store staging*/;
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -100,29 +101,39 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   tn = in / gsz;
 }
 
-template <int CG>
+// the four operand-layout combinations of one k-block (BK = 4 k-steps) of a warpgroup's 64 x BN tile
+template <int TA, int TB, int NB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[NB][64], uint32_t sa, uint32_t sb, bool first_kb) {
+  // K-major: a k-step of 16 bf16 advances the start address by 32 B inside the 128 B swizzle row;
+  // MN-major: by 16 k-rows x 128 B = 2 KB (descriptor address units are 16 B)
+  const uint64_t adesc = TA ? tc::wgmma_desc_sw128(sa, 8192, 1024) : tc::wgmma_desc_sw128(sa, 16, 1024);
+  const uint64_t bdesc = TB ? tc::wgmma_desc_sw128(sb, 8192, 1024) : tc::wgmma_desc_sw128(sb, 16, 1024);
+  constexpr uint64_t astep = TA ? 128 : 2, bstep = TB ? 128 : 2;
+  constexpr uint64_t bhalf = 16384 >> 4;     // columns 128.. of the B tile: 128 K-major rows or two MN-major chunks
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb)
+      tc::wgmma_m64n128k16_ss<TA, TB>(acc[nb], adesc + astep * k, bdesc + bstep * k + bhalf * nb, !(first_kb && k == 0));
+}
+
+template <int BN>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                         const GemmArgs g) {
-  using C_ = Cfg<CG>;
-  constexpr int STAGES = C_::STAGES;
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const GemmArgs g) {
+  using C_ = Cfg<BN>;
+  constexpr int STAGES = C_::STAGES, NB = BN / 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - tc::smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + STAGES * C_::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8 * s; };
   auto empty_bar = [&](int s) { return bar_base + 8 * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8 * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8 * (2 * STAGES + ACC + a); };
-  const uint32_t tmem_slot = bar_base + 8 * (2 * STAGES + 2 * ACC);
-  uint32_t* tmem_slot_gen = reinterpret_cast<uint32_t*>(smem_gen + STAGES * C_::STAGE_BYTES + 8 * (2 * STAGES + 2 * ACC));
-  float* s_bs = reinterpret_cast<float*>(smem_gen + STAGES * C_::STAGE_BYTES + 256);   // [2][bias BN | scale BN]
-  uint8_t* s_epi = reinterpret_cast<uint8_t*>(s_bs + 4 * BN);   // EPI_WARPS x 32 rows x EPI_PITCH bytes
+  float* s_bias = reinterpret_cast<float*>(smem_gen + STAGES * C_::STAGE_BYTES + 256);
+  float* s_scale = s_bias + BN;
+  uint8_t* s_epi = reinterpret_cast<uint8_t*>(s_scale + BN);   // CONSUMER_WARPS x 16 rows x EPI_PITCH bytes
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = CG == 2 ? tc::cluster_ctarank() : 0;
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x / CG, n_clusters = gridDim.x / CG;
   const int n_tiles = g.tiles_m * g.tiles_n;
   const int num_kb = (g.K + BK - 1) / BK;
 
@@ -131,28 +142,24 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
     tc::tma_prefetch_desc(&tmap_b);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), 1); }
-    for (int a = 0; a < ACC; ++a) { tc::mbar_init(tfull_bar(a), 1); tc::mbar_init(tempty_bar(a), EPI_WARPS * CG); }
+    for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), CONSUMER_WARPS); }
     tc::mbar_fence_init();
   }
-  if (warp == 2) tc::tmem_alloc<CG>(tmem_slot, ACC * BN);
-  tc::tc_fence_before();
-  if constexpr (CG == 2) tc::cluster_sync(); else __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_gen;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (tc::elect_one()) {
+    tc::reg_dealloc<40>();
+    if (warp == 0 && tc::elect_one()) {
       int stage = 0; uint32_t phase = 0;
-      for (int t = cluster_id; t < n_tiles; t += n_clusters) {
+      for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         int tm, tn; tile_coords(t, g.tiles_m, g.tiles_n, g.group_m, tm, tn);
-        const TilePlan tp = plan_tile(g, tm * CG * BM, tn * BN, CG * BM, num_kb);
+        const TilePlan tp = plan_tile(g, tm * BM, tn * BN, BM, num_kb);
         if (tp.skip) continue;
-        const int bt_m0 = g.bt_rows ? (tm * CG * BM) / g.bt_rows * g.bt_rows : 0;
+        const int bt_m0 = g.bt_rows ? (tm * BM) / g.bt_rows * g.bt_rows : 0;
         // K-major A: global stacked row; MN-major A: column inside its matrix (the stack runs along the K rows)
-        const int row_a = (tm * CG + (int)rank) * BM - (g.a_mn ? bt_m0 : 0);
-        const int row_b = tn * BN + (int)rank * C_::B_ROWS + (g.b_mn ? 0 : tp.b_row_off);
+        const int row_a = tm * BM - (g.a_mn ? bt_m0 : 0);
+        const int row_b = tn * BN + (g.b_mn ? 0 : tp.b_row_off);
         const int ka_off = g.a_mn ? tp.k_off : 0, kb_off = g.b_mn ? tp.k_off : 0;
         for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
           tc::mbar_wait(empty_bar(stage), phase ^ 1);
@@ -163,368 +170,188 @@ gemm_bf16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
             ka = (kb - seg * g.a_seg_kb) * BK;
             ra = row_a + seg * g.a_seg_rows;
           }
-          if constexpr (CG == 1) {
-            tc::mbar_arrive_expect_tx(full_bar(stage), C_::STAGE_BYTES);
-            if (g.a_mn) {
-              for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
-            } else {
-              tc::tma_load_2d(sa, &tmap_a, full_bar(stage), ka, ra);
-            }
-            if (g.b_mn) {
-              for (int h = 0; h < C_::B_ROWS / 64; ++h)
-                tc::tma_load_2d(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
-            } else {
-              tc::tma_load_2d(sb, &tmap_b, full_bar(stage), kb * BK, row_b);
-            }
+          tc::mbar_arrive_expect_tx(full_bar(stage), C_::STAGE_BYTES);
+          if (g.a_mn) {
+            for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
           } else {
-            if (leader) tc::mbar_arrive_expect_tx(full_bar(stage), 2 * C_::STAGE_BYTES);
-            if (g.a_mn) {
-              for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d_cg2(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
-            } else {
-              tc::tma_load_2d_cg2(sa, &tmap_a, full_bar(stage), ka, ra);
-            }
-            if (g.b_mn) {
-              for (int h = 0; h < C_::B_ROWS / 64; ++h)
-                tc::tma_load_2d_cg2(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
-            } else {
-              tc::tma_load_2d_cg2(sb, &tmap_b, full_bar(stage), kb * BK, row_b);
-            }
+            tc::tma_load_2d(sa, &tmap_a, full_bar(stage), ka, ra);
+          }
+          if (g.b_mn) {
+            for (int h = 0; h < BN / 64; ++h)
+              tc::tma_load_2d(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
+          } else {
+            tc::tma_load_2d(sb, &tmap_b, full_bar(stage), kb * BK, row_b);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA) =====================
-    if (leader) {
-      const uint32_t idesc = tc::umma_idesc_bf16_f32(BM * CG, BN) | (g.a_mn ? (1u << 15) : 0u) | (g.b_mn ? (1u << 16) : 0u);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-      for (int t = cluster_id; t < n_tiles; t += n_clusters) {
-        int tm_, tn_; tile_coords(t, g.tiles_m, g.tiles_n, g.group_m, tm_, tn_);
-        const TilePlan tp = plan_tile(g, tm_ * CG * BM, tn_ * BN, CG * BM, num_kb);
-        if (tp.skip) continue;
-        tc::mbar_wait(tempty_bar(acc), acc_phase ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
-          tc::mbar_wait(full_bar(stage), phase);
-          tc::tc_fence_after();
-          if (tc::elect_one()) {
-            const uint32_t sa = smem_base + stage * C_::STAGE_BYTES, sb = sa + A_BYTES;
-            // K-major: a k-step of 16 bf16 advances the start address by 32 B inside the 128 B swizzle row;
-            // MN-major: by 16 k-rows x 128 B = 2 KB (descriptor address units are 16 B)
-            const uint64_t adesc = g.a_mn ? tc::umma_desc_mnmajor_sw128(sa) : tc::umma_desc_kmajor_sw128(sa);
-            const uint64_t bdesc = g.b_mn ? tc::umma_desc_mnmajor_sw128(sb) : tc::umma_desc_kmajor_sw128(sb);
-            const uint64_t astep = g.a_mn ? 128 : 2, bstep = g.b_mn ? 128 : 2;
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k)
-              tc::umma_f16<CG>(d_tmem, adesc + astep * k, bdesc + bstep * k, idesc, (kb != tp.kb0) || (k != 0));
-            tc::umma_commit<CG>(empty_bar(stage));
-            if (kb == tp.kb1 - 1) tc::umma_commit<CG>(tfull_bar(acc));
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (++acc == ACC) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    // 8 epilogue warps: warp w reads TMEM lanes 32*(w%4).. (hardware rule); warps 4-7 take columns 0-127 of the
-    // tile, warps 8-11 columns 128-255, so a tile drains twice as fast (matters when K is short: GDINO K = 256)
-    const int quarter = warp & 3;
-    const int col_half = (warp - 4) >> 2;
-    const int et = threadIdx.x - 128;  // 0..255
-    int acc = 0; uint32_t acc_phase = 0;
-    const bool swiglu = g.act == ACT_SWIGLU;
-    // bias / column scale of a tile live in shared memory (broadcast reads in the epilogue math); the NEXT tile's slice is
-    // fetched into registers at the top of a tile and parked in the other buffer at its end, so the global-load latency
-    // (~1 us, as long as a whole K = 256 main loop) never sits between two tiles (static_assert: one element per thread)
-    static_assert(BN == 256, "one bias / scale element per epilogue thread");
-    int staged_tile = -1, buf = 0;
-    auto fetch_bs = [&](int tn_, float& b_, float& s_) {
-      const int col = tn_ * BN + et;
-      b_ = (g.bias && col < g.N) ? __bfloat162float(g.bias[col]) : 0.f;
-      s_ = (g.colscale && col < g.N) ? __bfloat162float(g.colscale[col]) : 1.f;
-    };
-    for (int t = cluster_id; t < n_tiles; t += n_clusters) {
-      int tm, tn; tile_coords(t, g.tiles_m, g.tiles_n, g.group_m, tm, tn);
-      if (plan_tile(g, tm * CG * BM, tn * BN, CG * BM, num_kb).skip) continue;
-      const int n0 = tn * BN;
-      const int row = (tm * CG + (int)rank) * BM + quarter * 32 + lane;
-      if (staged_tile != t) {                              // first tile (or the predicted successor was skipped)
-        float b0, s0; fetch_bs(tn, b0, s0);
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        s_bs[buf * 2 * BN + et] = b0; s_bs[buf * 2 * BN + BN + et] = s0;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
-      float* s_bias = s_bs + buf * 2 * BN;
-      float* s_scale = s_bias + BN;
-      const int t_next = t + n_clusters;
-      float nb = 0.f, ns = 1.f;
-      if (t_next < n_tiles) { int tm2, tn2; tile_coords(t_next, g.tiles_m, g.tiles_n, g.group_m, tm2, tn2); fetch_bs(tn2, nb, ns); }
-      tc::mbar_wait(tfull_bar(acc), acc_phase);
-      tc::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * BN;
-      const bool row_ok = row < g.M;
-      const bool zero_row = g.row_keep && row_ok && !g.row_keep[row];
-      // the 32-column step of the general path: direct row-per-thread stores (fp32 output, SwiGLU, ragged N)
-      auto direct32 = [&](int c) {
-        const int col0 = n0 + c;
-        if (col0 >= g.N) return;  // uniform
-        uint32_t r[32];
-        tc::tmem_ld_32x32(taddr + c, r);
-        tc::tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + s_bias[c + j];
-        if (g.act == ACT_GELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-        } else if (g.act == ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (g.act == ACT_SILU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = silu(v[j]);
-        } else if (g.act == ACT_QUICKGELU) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = v[j] / (1.f + __expf(-1.702f * v[j]));
-        }
-        if (swiglu) {
-          // columns (2j, 2j+1) = (gate, up) -> 16 outputs at column col0/2
-          if (row_ok) {
-            const int oc0 = col0 >> 1;
-            const int n_out = g.N >> 1;
-            float o[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) o[j] = silu(v[2 * j]) * v[2 * j + 1];
-            if (g.residual) {
-              const __nv_bfloat16* rp = g.residual + (size_t)row * g.ldr + oc0;
-#pragma unroll
-              for (int j = 0; j < 16; ++j) if (oc0 + j < n_out) o[j] += __bfloat162float(rp[j]);
-            }
-            __nv_bfloat16* cp = reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc + oc0;
-            if (oc0 + 16 <= n_out) {
-#pragma unroll
-              for (int q = 0; q < 2; ++q) {
-                uint4 pk;
-                __nv_bfloat162 p0 = __floats2bfloat162_rn(o[8 * q + 0], o[8 * q + 1]);
-                __nv_bfloat162 p1 = __floats2bfloat162_rn(o[8 * q + 2], o[8 * q + 3]);
-                __nv_bfloat162 p2 = __floats2bfloat162_rn(o[8 * q + 4], o[8 * q + 5]);
-                __nv_bfloat162 p3 = __floats2bfloat162_rn(o[8 * q + 6], o[8 * q + 7]);
-                pk.x = *reinterpret_cast<uint32_t*>(&p0); pk.y = *reinterpret_cast<uint32_t*>(&p1);
-                pk.z = *reinterpret_cast<uint32_t*>(&p2); pk.w = *reinterpret_cast<uint32_t*>(&p3);
-                *reinterpret_cast<uint4*>(cp + 8 * q) = pk;
-              }
-            } else {
-              for (int j = 0; j < 16; ++j) if (oc0 + j < n_out) cp[j] = __float2bfloat16(o[j]);
-            }
-          }
-          return;
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] *= s_scale[c + j];
-        if (row_ok) {
-          const bool full = col0 + 32 <= g.N;
-          if (g.residual) {
-            const __nv_bfloat16* rp = g.residual + (size_t)row * g.ldr + col0;
-            if (full) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint4 rr = *reinterpret_cast<const uint4*>(rp + 8 * q);
-                const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rr);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const float2 f = __bfloat1622float2(r2[j]);
-                  v[8 * q + 2 * j] += f.x; v[8 * q + 2 * j + 1] += f.y;
-                }
-              }
-            } else {
-              for (int j = 0; j < 32; ++j) if (col0 + j < g.N) v[j] += __bfloat162float(rp[j]);
-            }
-          }
-          if (zero_row) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = 0.f;
-          }
-          if (g.out_f32) {
-            float* cp = reinterpret_cast<float*>(g.C) + (size_t)row * g.ldc + col0;
-            if (full) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q)
-                *reinterpret_cast<float4*>(cp + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            } else {
-              for (int j = 0; j < 32; ++j) if (col0 + j < g.N) cp[j] = v[j];
-            }
-          } else {
-            __nv_bfloat16* cp = reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc + col0;
-            if (full) {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                uint4 pk;
-                __nv_bfloat162 p0 = __floats2bfloat162_rn(v[8 * q + 0], v[8 * q + 1]);
-                __nv_bfloat162 p1 = __floats2bfloat162_rn(v[8 * q + 2], v[8 * q + 3]);
-                __nv_bfloat162 p2 = __floats2bfloat162_rn(v[8 * q + 4], v[8 * q + 5]);
-                __nv_bfloat162 p3 = __floats2bfloat162_rn(v[8 * q + 6], v[8 * q + 7]);
-                pk.x = *reinterpret_cast<uint32_t*>(&p0); pk.y = *reinterpret_cast<uint32_t*>(&p1);
-                pk.z = *reinterpret_cast<uint32_t*>(&p2); pk.w = *reinterpret_cast<uint32_t*>(&p3);
-                *reinterpret_cast<uint4*>(cp + 8 * q) = pk;
-              }
-            } else {
-              for (int j = 0; j < 32; ++j) if (col0 + j < g.N) cp[j] = __float2bfloat16(v[j]);
-            }
-          }
-        }
-            };
-      uint8_t* my_stage = s_epi + (warp - 4) * EPI_STAGE_BYTES;
-#pragma unroll 1
-      for (int c = col_half * (BN / 2); c < (col_half + 1) * (BN / 2); c += 64) {
-        const int col0 = n0 + c;
-        if (col0 >= g.N) break;  // uniform
-        if (swiglu || g.out_f32 || col0 + 64 > g.N) { direct32(c); direct32(c + 32); continue; }
-        // ---- bf16 fast path: stage 32 rows x 64 columns per warp in smem, then store 128-byte row runs ----
-        auto half = [&](const uint32_t (&r)[32], const int h) {
-          float v[32];
-          if (g.bias) {                      // 16-byte broadcast reads: 8 LDS.128 instead of 32 LDS.32
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 b4 = *reinterpret_cast<const float4*>(&s_bias[c + 32 * h + 4 * q]);
-              v[4 * q] = __uint_as_float(r[4 * q]) + b4.x; v[4 * q + 1] = __uint_as_float(r[4 * q + 1]) + b4.y;
-              v[4 * q + 2] = __uint_as_float(r[4 * q + 2]) + b4.z; v[4 * q + 3] = __uint_as_float(r[4 * q + 3]) + b4.w;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-          }
-          if (g.act == ACT_GELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-          } else if (g.act == ACT_RELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (g.act == ACT_SILU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = silu(v[j]);
-          } else if (g.act == ACT_QUICKGELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = v[j] / (1.f + __expf(-1.702f * v[j]));
-          }
-          if (g.colscale) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 s4 = *reinterpret_cast<const float4*>(&s_scale[c + 32 * h + 4 * q]);
-              v[4 * q] *= s4.x; v[4 * q + 1] *= s4.y; v[4 * q + 2] *= s4.z; v[4 * q + 3] *= s4.w;
-            }
-          }
-          if (g.residual && row_ok) {
-            const __nv_bfloat16* rp = g.residual + (size_t)row * g.ldr + col0 + 32 * h;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint4 rr = *reinterpret_cast<const uint4*>(rp + 8 * q);
-              const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rr);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float2 f = __bfloat1622float2(r2[j]);
-                v[8 * q + 2 * j] += f.x; v[8 * q + 2 * j + 1] += f.y;
-              }
-            }
-          }
-          if (zero_row) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = 0.f;
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 pk;
-            __nv_bfloat162 p0 = __floats2bfloat162_rn(v[8 * q + 0], v[8 * q + 1]);
-            __nv_bfloat162 p1 = __floats2bfloat162_rn(v[8 * q + 2], v[8 * q + 3]);
-            __nv_bfloat162 p2 = __floats2bfloat162_rn(v[8 * q + 4], v[8 * q + 5]);
-            __nv_bfloat162 p3 = __floats2bfloat162_rn(v[8 * q + 6], v[8 * q + 7]);
-            pk.x = *reinterpret_cast<uint32_t*>(&p0); pk.y = *reinterpret_cast<uint32_t*>(&p1);
-            pk.z = *reinterpret_cast<uint32_t*>(&p2); pk.w = *reinterpret_cast<uint32_t*>(&p3);
-            *reinterpret_cast<uint4*>(my_stage + lane * EPI_PITCH + h * 64 + q * 16) = pk;
-          }
-                };
-        {
-          uint32_t r0[32], r1[32];
-          tc::tmem_ld_32x32(taddr + c, r0);
-          tc::tmem_ld_wait();
-          tc::tmem_ld_32x32(taddr + c + 32, r1);     // in flight while the first half is processed
-          half(r0, 0);
-          tc::tmem_ld_wait();
-          half(r1, 1);
-        }
-        __syncwarp();
-        {
-          const int row_base = (tm * CG + (int)rank) * BM + quarter * 32;
-          __nv_bfloat16* cbase = reinterpret_cast<__nv_bfloat16*>(g.C) + col0;
-          int row_local = row_base;
-          if (g.sc_rows && row_base < g.M) {         // peer push: the 32 rows of a warp share one destination
-            const int d = row_base / g.sc_rows;
-            cbase = reinterpret_cast<__nv_bfloat16*>(g.sc_dst[d]) + col0;
-            row_local = row_base - d * g.sc_rows;
-          }
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {           // each instruction: 4 rows x 128 contiguous bytes
-            const int rr = it * 4 + (lane >> 3), piece = lane & 7;
-            const uint4 val = *reinterpret_cast<const uint4*>(my_stage + rr * EPI_PITCH + piece * 16);
-            if (row_base + rr < g.M)
-              *reinterpret_cast<uint4*>(cbase + (size_t)(row_local + rr) * g.ldc + piece * 8) = val;
-          }
-        }
-        __syncwarp();
-      }
-      // accumulator stage drained: hand it back to the MMA issuer
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 1) tc::mbar_arrive(tempty_bar(acc));
-        else tc::mbar_arrive_cluster(tempty_bar(acc), 0);
-      }
-      if (g.sc_rows) {                               // tile pushed: publish it to the owner of these rows (after the
-        const int row_base = (tm * CG + (int)rank) * BM + quarter * 32;   // TMEM hand-back: the fence waits for NVLink acks)
-        __threadfence_system();
-        __syncwarp();
-        if (lane == 0 && row_base < g.M)
-          asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(g.sc_flag[row_base / g.sc_rows]), "r"(1u) : "memory");
-      }
-      if (++acc == ACC) { acc = 0; acc_phase ^= 1; }
-      if (t_next < n_tiles) {                              // park the successor's bias / scale (nobody reads that buffer now)
-        s_bs[(buf ^ 1) * 2 * BN + et] = nb; s_bs[(buf ^ 1) * 2 * BN + BN + et] = ns;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        staged_tile = t_next; buf ^= 1;
-      }
-    }
+    return;
   }
 
-  // ===================== teardown =====================
-  tc::tc_fence_before();
-  if constexpr (CG == 2) tc::cluster_sync(); else __syncthreads();
-  if (warp == 2) tc::tmem_dealloc<CG>(tmem_base, ACC * BN);
+  // ===================== consumers: main loop + epilogue =====================
+  tc::reg_alloc<232>();
+  const int wg = (warp - 4) >> 2;                  // 0 / 1: rows 0-63 / 64-127 of the tile
+  const int et = threadIdx.x - 128;                // 0..255
+  const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
+  const bool swiglu = g.act == ACT_SWIGLU;
+  int stage = 0; uint32_t phase = 0;
+  float acc[NB][64];
+  for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    int tm, tn; tile_coords(t, g.tiles_m, g.tiles_n, g.group_m, tm, tn);
+    const TilePlan tp = plan_tile(g, tm * BM, tn * BN, BM, num_kb);
+    if (tp.skip) continue;
+    const int n0 = tn * BN;
+    // bias / column scale of the tile go to shared memory now (broadcast reads in the epilogue math), so their global-load
+    // latency hides under the main loop; the previous tile's readers left at the barrier that closed its epilogue
+    if (et < BN) {
+      const int col = n0 + et;
+      s_bias[et] = (g.bias && col < g.N) ? __bfloat162float(g.bias[col]) : 0.f;
+      s_scale[et] = (g.colscale && col < g.N) ? __bfloat162float(g.colscale[col]) : 1.f;
+    }
+    int prev_stage = -1;
+    for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
+      tc::mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = smem_base + stage * C_::STAGE_BYTES + wg * 8192, sb = smem_base + stage * C_::STAGE_BYTES + A_BYTES;
+      const bool first = kb == tp.kb0;
+#pragma unroll
+      for (int nb = 0; nb < NB; ++nb) tc::acc_fence(acc[nb]);
+      tc::wgmma_fence();
+      if (g.a_mn) {
+        if (g.b_mn) mma_kblock<1, 1, NB>(acc, sa, sb, first); else mma_kblock<1, 0, NB>(acc, sa, sb, first);
+      } else {
+        if (g.b_mn) mma_kblock<0, 1, NB>(acc, sa, sb, first); else mma_kblock<0, 0, NB>(acc, sa, sb, first);
+      }
+      tc::wgmma_commit();
+      tc::wgmma_wait<1>();                           // the previous k-block's MMAs have retired: its stage is free
+      if (prev_stage >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev_stage));
+      prev_stage = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb) tc::acc_fence(acc[nb]);
+    if (lane == 0) tc::mbar_arrive(empty_bar(prev_stage));
+    tc::named_bar_sync(1, CONSUMER_THREADS);         // s_bias / s_scale of this tile are in place
+
+    // ---- epilogue on the accumulator fragments: element pair (c, c + 1) of rows r and r + 8 per n8 block ----
+    // bias -> activation -> column scale -> residual -> row mask on the pair (c, c + 1) of `row` (not for SwiGLU)
+    auto math = [&](int row, int c, float& v0, float& v1) {
+      const int col = n0 + c;
+      v0 += s_bias[c]; v1 += s_bias[c + 1];
+      if (g.act == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+      else if (g.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      else if (g.act == ACT_SILU) { v0 = silu(v0); v1 = silu(v1); }
+      else if (g.act == ACT_QUICKGELU) { v0 = v0 / (1.f + __expf(-1.702f * v0)); v1 = v1 / (1.f + __expf(-1.702f * v1)); }
+      v0 *= s_scale[c]; v1 *= s_scale[c + 1];
+      if (row >= g.M) return;
+      if (g.residual) {
+        const __nv_bfloat16* rp = g.residual + (size_t)row * g.ldr + col;
+        if (col + 1 < g.N) {                         // col is even: a pair is 4-byte aligned
+          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rp));
+          v0 += f.x; v1 += f.y;
+        } else {
+          v0 += __bfloat162float(rp[0]);
+        }
+      }
+      if (g.row_keep && !g.row_keep[row]) { v0 = 0.f; v1 = 0.f; }
+    };
+    // destination of an output row: C, or the peer slot that owns row block d of C (scatter mode)
+    auto out_row = [&](int row) -> __nv_bfloat16* {
+      if (!g.sc_rows) return reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc;
+      const int d = row / g.sc_rows;
+      return reinterpret_cast<__nv_bfloat16*>(g.sc_dst[d]) + (size_t)(row - d * g.sc_rows) * g.ldc;
+    };
+    // general path: the pair goes straight from the fragment to global memory (fp32 output, SwiGLU, ragged N)
+    auto emit = [&](int row, int c, float v0, float v1) {
+      const int col = n0 + c;
+      if (row >= g.M || col >= g.N) return;
+      if (swiglu) {                                  // columns (2j, 2j+1) = (gate, up) -> output column j
+        const int oc = col >> 1;
+        float o = silu(v0 + s_bias[c]) * (v1 + s_bias[c + 1]);
+        if (g.residual) o += __bfloat162float(g.residual[(size_t)row * g.ldr + oc]);
+        reinterpret_cast<__nv_bfloat16*>(g.C)[(size_t)row * g.ldc + oc] = __float2bfloat16(o);
+        return;
+      }
+      math(row, c, v0, v1);
+      const bool pair = col + 1 < g.N;               // 4-byte (bf16) / 8-byte (fp32) aligned
+      if (g.out_f32) {
+        float* cp = reinterpret_cast<float*>(g.C) + (size_t)row * g.ldc + col;
+        if (pair) *reinterpret_cast<float2*>(cp) = make_float2(v0, v1); else cp[0] = v0;
+        return;
+      }
+      __nv_bfloat16* cp = out_row(row) + col;
+      if (pair) *reinterpret_cast<__nv_bfloat162*>(cp) = __floats2bfloat162_rn(v0, v1); else cp[0] = __float2bfloat16(v0);
+    };
+    const int row0 = tm * BM + frag_row;
+    const int warp_row0 = tm * BM + wg * 64 + (warp & 3) * 16;
+    uint8_t* my_stage = s_epi + (warp - 4) * EPI_WARP_BYTES;
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb) {
+#pragma unroll
+      for (int ch = 0; ch < 2; ++ch) {               // 64-column chunks of this 128-column accumulator half
+        const int c0 = nb * 128 + ch * 64;
+        if (n0 + c0 >= g.N) break;                   // uniform
+        if (swiglu || g.out_f32 || n0 + c0 + 64 > g.N) {
+#pragma unroll
+          for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
+            const int c = nb * 128 + 8 * j + frag_col;
+            emit(row0, c, acc[nb][4 * j], acc[nb][4 * j + 1]);
+            emit(row0 + 8, c, acc[nb][4 * j + 2], acc[nb][4 * j + 3]);
+          }
+          continue;
+        }
+        // bf16 fast path: the warp stages its 16 rows x 64 columns in shared memory, then stores 128-byte row runs
+        // (4-byte stores from the fragments would cost the L2 eight requests per 128-byte line instead of one)
+#pragma unroll
+        for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
+          const int c = nb * 128 + 8 * j + frag_col;
+          float a0 = acc[nb][4 * j], a1 = acc[nb][4 * j + 1], b0 = acc[nb][4 * j + 2], b1 = acc[nb][4 * j + 3];
+          math(row0, c, a0, a1);
+          math(row0 + 8, c, b0, b1);
+          const int off = (8 * (j - 8 * ch) + frag_col) * 2;
+          *reinterpret_cast<__nv_bfloat162*>(my_stage + (lane >> 2) * EPI_PITCH + off) = __floats2bfloat162_rn(a0, a1);
+          *reinterpret_cast<__nv_bfloat162*>(my_stage + ((lane >> 2) + 8) * EPI_PITCH + off) = __floats2bfloat162_rn(b0, b1);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int it = 0; it < 4; ++it) {             // each instruction: 4 rows x 128 contiguous bytes
+          const int rr = it * 4 + (lane >> 3), piece = lane & 7;
+          const uint4 val = *reinterpret_cast<const uint4*>(my_stage + rr * EPI_PITCH + piece * 16);
+          if (warp_row0 + rr < g.M) *reinterpret_cast<uint4*>(out_row(warp_row0 + rr) + n0 + c0 + piece * 8) = val;
+        }
+        __syncwarp();
+      }
+    }
+    if (g.sc_rows) {                                 // tile pushed: publish it to the owner of these rows
+      __threadfence_system();
+      __syncwarp();
+      if (lane == 0 && warp_row0 < g.M)
+        asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(g.sc_flag[warp_row0 / g.sc_rows]), "r"(1u) : "memory");
+    }
+    tc::named_bar_sync(1, CONSUMER_THREADS);         // every reader of s_bias / s_scale is done: the next tile may overwrite
+  }
 }
 
-// Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so a wave
-// of 74 CTA pairs covers ~8 x 9 tiles (near-square = minimal A+B bytes per wave).  Measured (profiles/
-// r1_gemm_raster_experiment.md): DRAM traffic and ncu durations move by < 3 % between group sizes 1..8 at the
-// ViT shapes and get worse below 8 for the wide LLM gate|up GEMM, so 8 stays; the knob remains for sweeps.
+// Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so one wave of
+// CTAs covers a near-square patch of tiles (minimal A+B bytes per wave).  The knob remains for sweeps.
 int g_group_m_override = 0;
-// SM budgets (0 = every SM): a persistent GEMM CTA owns its SM (168 registers x 384 threads = the whole register file), so a
+// SM budgets (0 = every SM): a persistent GEMM CTA owns its SM (384 threads with the whole register file between them), so a
 // link-bound kernel of another stream -- the peer pushes of the tensor-parallel exchange -- can only overlap a GEMM on SMs
 // the GEMM's grid leaves free.  g_sm_limit caps every launch, g_scatter_sm_limit the scatter GEMM (vllm_gemm_bf16_scatter),
 // whose epilogue stores ride NVLink while the other micro-batch's GEMM runs beside it (visionllm_b200/tp.py).
 int g_sm_limit = 0, g_scatter_sm_limit = 0;
 int pick_group_m(int, int, long long) { return g_group_m_override > 0 ? g_group_m_override : 8; }
 
-// 0: auto (cta_group::2 CTA pairs, 256x256 tiles; cta_group::1 when K <= 512, where the cross-CTA hand-offs of
-// a pair cost more than the halved B traffic saves: 617 vs 494 TFLOP/s at K = 256); 1 / 2: force
+// 0: auto = 128 x 128 tiles (faster than 128 x 256 at every hot-path shape measured on an H100, README.md);
+// 1 / 2: force the 128- / 256-column tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its receivers
+// count arrivals per such tile.
 int g_gemm_variant = 0;
 
-template <int CG>
+template <int BN>
 int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cudaStream_t st, long long a_rows = -1,
                 int a_cols = -1) {
-  using C_ = Cfg<CG>;
+  using C_ = Cfg<BN>;
   CUtensorMap ta, tb;
   const uint64_t nb = g.bt_rows ? (uint64_t)(g.M / g.bt_rows) : 1;     // matrices in the stack (batched mode)
   const uint64_t m_local = g.bt_rows ? (uint64_t)g.bt_rows : (uint64_t)g.M;
@@ -533,36 +360,33 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
                                         (uint64_t)(a_cols < 0 ? g.K : a_cols), (uint64_t)lda, BM);
   if (rc) return rc;
   rc = g.b_mn ? vllm_make_tmap_bf16(&tb, B, nb * (uint64_t)g.K, (uint64_t)g.N, (uint64_t)ldb, 64)
-              : vllm_make_tmap_bf16(&tb, B, nb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, C_::B_ROWS);
+              : vllm_make_tmap_bf16(&tb, B, nb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, BN);
   if (rc) return rc;
-  g.tiles_m = (g.M + BM * CG - 1) / (BM * CG);
+  g.tiles_m = (g.M + BM - 1) / BM;
   g.tiles_n = (g.N + BN - 1) / BN;
   const int n_tiles = g.tiles_m * g.tiles_n;
   int sms = vllm_num_sms();
   const int limit = g.sc_rows ? (g_scatter_sm_limit > 0 ? g_scatter_sm_limit : g_sm_limit) : g_sm_limit;
-  if (limit > 0 && limit < sms) sms = limit < CG ? CG : limit;
-  int clusters = sms / CG;
-  if (clusters > n_tiles) clusters = n_tiles;
-  g.group_m = pick_group_m(sms / CG, g.tiles_n, (long long)g.N * g.K * 2);
-  static bool attr_set[3] = {false, false, false};
-  if (!attr_set[CG]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_tcgen05_kernel<CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         C_::SMEM);
+  if (limit > 0 && limit < sms) sms = limit;
+  const int ctas = sms < n_tiles ? sms : n_tiles;
+  g.group_m = pick_group_m(sms, g.tiles_n, (long long)g.N * g.K * 2);
+  static bool attr_set[64] = {false};
+  bool* set = vllm_device_flag(attr_set);
+  if (!set || !*set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM);
     if (e != cudaSuccess) return (int)e;
-    attr_set[CG] = true;
+    if (set) *set = true;
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(clusters * CG);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = C_::SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_bf16_tcgen05_kernel<CG>, ta, tb, g);
-  if (e != cudaSuccess) return (int)e;
+  gemm_bf16_wgmma_kernel<BN><<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, g);
+  VLLM_CHECK_LAUNCH();
   return VLLM_OK;
+}
+
+int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmArgs& g, cudaStream_t st, long long a_rows = -1,
+                     int a_cols = -1) {
+  // the receivers of a scatter GEMM count 8 arrivals per 128 x 256 tile (visionllm_b200/tp.py)
+  const bool wide = g.sc_rows || g_gemm_variant == 2;
+  return wide ? launch_gemm<256>(A, lda, B, ldb, g, st, a_rows, a_cols) : launch_gemm<128>(A, lda, B, ldb, g, st, a_rows, a_cols);
 }
 
 }  // namespace
@@ -615,9 +439,7 @@ static int gemm_bf16_common(const void* A, int lda, const void* B, int ldb, void
   g.residual = (const __nv_bfloat16*)residual; g.ldr = ldr; g.act = act; g.out_f32 = out_f32;
   g.row_keep = row_keep;
   cudaStream_t st = (cudaStream_t)stream;
-  const int cg = g_gemm_variant ? g_gemm_variant : (K <= 512 ? 1 : 2);
-  if (cg == 2) return launch_gemm<2>(A, lda, B, ldb, g, st);
-  return launch_gemm<1>(A, lda, B, ldb, g, st);
+  return launch_gemm_auto(A, lda, B, ldb, g, st);
 }
 
 int vllm_gemm_bf16_tn(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc, int M,
@@ -636,9 +458,7 @@ int vllm_gemm_bf16_tn(const void* A, int lda, int a_mn_major, const void* B, int
   g.M = M; g.N = N; g.K = K; g.C = C; g.ldc = ldc; g.out_f32 = out_f32;
   g.a_mn = a_mn_major ? 1 : 0; g.b_mn = b_mn_major ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
-  const int cg = g_gemm_variant ? g_gemm_variant : (K <= 512 ? 1 : 2);
-  if (cg == 2) return launch_gemm<2>(A, lda, B, ldb, g, st);
-  return launch_gemm<1>(A, lda, B, ldb, g, st);
+  return launch_gemm_auto(A, lda, B, ldb, g, st);
 }
 
 int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc,
@@ -647,6 +467,8 @@ int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B
   // n_batch matrices along the row axis (K-major A: [n_batch*M, K]; MN-major A: [n_batch*K, M]; same for B; C: [n_batch*M, N]).
   // causal (square attention matrices, M == the sequence length): see GemmArgs.  The attention-backward GEMMs of a layer.
   if (n_batch < 0 || M <= 0 || N <= 0 || K <= 0 || causal < 0 || causal > 3) return VLLM_EINVAL;
+  if (causal >= 2 && K != M) return VLLM_EINVAL;     // modes 2 / 3 cut the K axis at the tile's rows: K is the sequence axis, and
+                                                     // with K == M (a multiple of 256) every tile keeps at least one k-block
   if (n_batch == 0) return VLLM_OK;
   if (!A || !B || !C) return VLLM_EINVAL;
   if (M % 256 || ((a_mn_major || b_mn_major) && K % BK)) return VLLM_EUNSUPPORTED;     // tiles must not straddle matrices
@@ -660,18 +482,16 @@ int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B
   g.a_mn = a_mn_major ? 1 : 0; g.b_mn = b_mn_major ? 1 : 0;
   g.bt_rows = M; g.causal = causal;
   cudaStream_t st = (cudaStream_t)stream;
-  const int cg = g_gemm_variant ? g_gemm_variant : (K <= 512 ? 1 : 2);
-  if (cg == 2) return launch_gemm<2>(A, lda, B, ldb, g, st);
-  return launch_gemm<1>(A, lda, B, ldb, g, st);
+  return launch_gemm_auto(A, lda, B, ldb, g, st);
 }
 
 int vllm_gemm_bf16_scatter(const void* A, int lda, const void* B, int ldb, void* const* dst, void* const* flags,
                            int n_dst, int rows_per_dst, int ldc, int N, int K, void* stream) {
   // C = A . B^T (plain bf16, no epilogue math), M = n_dst * rows_per_dst; row block d is stored to dst[d] and
-  // counted on flags[d] (8 arrivals per 128 x 256 tile: (rows_per_dst / 128) * ceil(N / 256) * 8 per source and pass).
+  // counted on flags[d] (8 arrivals, one per consumer warp, per 128 x 256 tile: (rows_per_dst / 128) * ceil(N / 256) * 8 per source and pass).
   if (n_dst <= 0 || n_dst > 8 || rows_per_dst <= 0 || N <= 0 || K <= 0 || lda < K || ldb < K || ldc < N) return VLLM_EINVAL;
   if (!A || !B || !dst || !flags) return VLLM_EINVAL;
-  if (rows_per_dst % BM || N % 64) return VLLM_EUNSUPPORTED;    // a warp's 32 rows share a destination; bf16 fast path
+  if (rows_per_dst % BM || N % 64) return VLLM_EUNSUPPORTED;    // a tile's rows share a destination; bf16 column pairs
   if ((long long)n_dst * rows_per_dst > 2147483647LL) return VLLM_EUNSUPPORTED;
   if (!vllm_aligned(A, 16) || !vllm_aligned(B, 16) || (lda % 8) || (ldb % 8) || (ldc % 8)) return VLLM_EALIGN;
   GemmArgs g{};
@@ -683,9 +503,7 @@ int vllm_gemm_bf16_scatter(const void* A, int lda, const void* B, int ldb, void*
   }
   g.C = dst[0];
   cudaStream_t st = (cudaStream_t)stream;
-  const int cg = g_gemm_variant ? g_gemm_variant : (K <= 512 ? 1 : 2);
-  if (cg == 2) return launch_gemm<2>(A, lda, B, ldb, g, st);
-  return launch_gemm<1>(A, lda, B, ldb, g, st);
+  return launch_gemm_auto(A, lda, B, ldb, g, st);
 }
 
 int vllm_conv_rows_bf16(const void* xpad, long long pad_pixels, int channels, int padded_width, int kernel_h,
@@ -710,9 +528,7 @@ int vllm_conv_rows_bf16(const void* xpad, long long pad_pixels, int channels, in
   g.bias = (const __nv_bfloat16*)bias; g.act = act;
   g.a_seg_kb = (int)(seg_k / BK); g.a_seg_rows = padded_width;
   cudaStream_t st = (cudaStream_t)stream;
-  const int cg = g_gemm_variant ? g_gemm_variant : (g.K <= 512 ? 1 : 2);
-  if (cg == 2) return launch_gemm<2>(xpad, channels, weight, ldw, g, st, a_rows, (int)seg_k);
-  return launch_gemm<1>(xpad, channels, weight, ldw, g, st, a_rows, (int)seg_k);
+  return launch_gemm_auto(xpad, channels, weight, ldw, g, st, a_rows, (int)seg_k);
 }
 
 }  // extern "C"

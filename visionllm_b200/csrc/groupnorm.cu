@@ -105,8 +105,8 @@ __global__ void __launch_bounds__(GN_THREADS) gn_apply_kernel(const __nv_bfloat1
   const float2 st = stat[(oct * 8) / cpg];
   const uint4* xin = reinterpret_cast<const uint4*>(x + (long long)n * img_pitch * c) + oct;
   uint4* yout = reinterpret_cast<uint4*>(y + (long long)n * hw * c) + oct;
-  // four pixels per thread and iteration: four independent 16-byte loads in flight (one load per iteration left the apply pass
-  // latency-bound at 1.7 TB/s on the 256 x 256 x 256 maps, ncu r2_glue_kernels_ncu.json)
+  // four pixels per thread and iteration: four independent 16-byte loads in flight (one load per iteration leaves the apply
+  // pass latency-bound)
   const long long step = (long long)gridDim.x * ppi;
   for (long long p0 = (long long)blockIdx.x * ppi + prow; p0 < hw; p0 += 4 * step) {
     uint4 raw[4];

@@ -1,4 +1,4 @@
-// Multi-scale deformable attention (MSDA) forward for sm_100a.
+// Multi-scale deformable attention (MSDA) forward for sm_90a.
 //
 // Replaces the reference operator
 //   mmcv/ops/csrc/common/cuda/ms_deform_attn_cuda_kernel.cuh:17-64,200-254
@@ -354,11 +354,7 @@ msda_pack_pairs_kernel(const __nv_bfloat16* __restrict__ value, __nv_bfloat16* _
 
 constexpr int MSDA_PAIR_ROW = 32 + 2;   // int2 entries per (warp, row, column) slab: 32 samples + pad (slabs on different banks)
 
-// FH (experimental, vllm_msda_set_variant(16), not validated on hardware yet): the per-corner weight is rounded to bf16
-// and the products run on sm_100a's mixed-precision FMA (`fma.rn.f32.bf16` = SASS FHFMA.BF16 with .H0/.H1 selectors,
-// fp32 accumulate), which consumes the packed bf16 value halves directly -- no unpack instructions (64 of the ~340 per
-// (query, head)); the bf16 x bf16 product is exact, the only new error is the 2^-9 rounding of each corner weight.
-template <int TH, int TW, int NW, int KC, int PC, typename OutT, bool FH = false>
+template <int TH, int TW, int NW, int KC, int PC, typename OutT>
 __global__ void __launch_bounds__(NW * 32)
 msda_fwd_pair_kernel(const __nv_bfloat16* __restrict__ pairs, const int64_t* __restrict__ shapes,
                      const int64_t* __restrict__ lsi, const float* __restrict__ loc,
@@ -454,22 +450,12 @@ msda_fwd_pair_kernel(const __nv_bfloat16* __restrict__ pairs, const int64_t* __r
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = 0.f;
       auto fma8 = [&](const uint4& raw, float w) {
-        if constexpr (FH) {
-          const uint32_t wb = (uint32_t)__bfloat16_as_ushort(__float2bfloat16(w));
-          const uint32_t words[4] = {raw.x, raw.y, raw.z, raw.w};
+        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&raw);
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            asm("{\n\t.reg .b16 xl, xh, wl, wh;\n\tmov.b32 {xl, xh}, %2;\n\tmov.b32 {wl, wh}, %3;\n\t"
-                "fma.rn.f32.bf16 %0, xl, wl, %0;\n\tfma.rn.f32.bf16 %1, xh, wl, %1;\n\t}"
-                : "+f"(acc[2 * i]), "+f"(acc[2 * i + 1]) : "r"(words[i]), "r"(wb));
-        } else {
-          const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 f = __bfloat1622float2(h[i]);
-            acc[2 * i] = fmaf(w, f.x, acc[2 * i]);
-            acc[2 * i + 1] = fmaf(w, f.y, acc[2 * i + 1]);
-          }
+        for (int i = 0; i < 4; ++i) {
+          const float2 f = __bfloat1622float2(h[i]);
+          acc[2 * i] = fmaf(w, f.x, acc[2 * i]);
+          acc[2 * i + 1] = fmaf(w, f.y, acc[2 * i + 1]);
         }
       };
       if constexpr (KC > 0 && (KC / 2) % 4 == 0) {
@@ -661,10 +647,7 @@ static int launch_pair(const __nv_bfloat16* pairs, const int64_t* shapes, const 
   build_tiling(tl, host_shapes, L, Lq, S, TH, TW);
   dim3 grid((unsigned)(tl.n_tiles * M), (unsigned)N);
   if (N > 65535) return VLLM_EUNSUPPORTED;
-  if (L == 4 && P == 4 && g_msda_variant == 16)
-    msda_fwd_pair_kernel<TH, TW, NW, 16, 4, OutT, true><<<grid, NW * 32, 0, st>>>(pairs, shapes, lsi, loc, attw, out, S,
-                                                                                  M, L, Lq, P, tl);
-  else if (L == 4 && P == 4)
+  if (L == 4 && P == 4)
     msda_fwd_pair_kernel<TH, TW, NW, 16, 4, OutT><<<grid, NW * 32, 0, st>>>(pairs, shapes, lsi, loc, attw, out, S, M, L,
                                                                             Lq, P, tl);
   else
@@ -716,8 +699,8 @@ int vllm_msda_forward_f32(const float* value, const int64_t* spatial_shapes, con
   if (!strict && channels == 32 && K <= 32 && vllm_aligned(value, 16) && vllm_aligned(out, 16) &&
       vllm_aligned(sampling_loc, 8)) {
     // encoder shape, fp32 rows: the TMA-staged window kernel (msda_win.cu) is opt-in (variant 33) -- 128-byte rows leave
-    // room for an 8 x 8 patch only and it measures 0.62 ms against 0.59 ms for the global-memory patch kernel below
-    // (profiles/r2_msda_window_sweep.json); bf16 rows (vllm_msda_forward_bf16v) take the window kernel by default
+    // room for an 8 x 8 patch only (not re-measured on the H100 against the global-memory patch kernel below);
+    // bf16 rows (vllm_msda_forward_bf16v) take the window kernel by default
     if (g_msda_variant == 33) {
       const int r = msda_launch_window<float, float>(value, level_start_index, sampling_loc, attn_weight, out, batch,
                                                      spatial_size, num_heads, num_levels, num_query, num_point,

@@ -4,9 +4,9 @@
 // unipose/ops/src/cuda/ms_deform_im2col_cuda.cuh:237-300); entered from vllm_msda_forward_bf16v / _f32 when the
 // caller's host-side shape hint proves that the queries are the pixels of the pyramid.
 //
-// Why: the gather is bound by L1 wavefronts, not by HBM bytes (tools/gather_ceiling.cu: 0.95 rows of 128 B per clock
-// per SM through L1 or shared memory, whatever the hit rate).  Through L1 a 64-byte bf16 row costs as much as a
-// 128-byte fp32 row (one tag / one line per row); from shared memory it costs half (1.93 rows / clk / SM measured).
+// Why: the gather is bound by L1 wavefronts, not by HBM bytes.  Through L1 a 64-byte bf16 row costs as much as a
+// 128-byte fp32 row (one tag / one line per row); from shared memory it costs half.  (The rates behind this design were
+// measured on another architecture and have not been re-measured on the H100.)
 // So: one CTA owns a REGION of the image (a PH x PW patch of level-0 pixels and the pixels of every other level whose
 // centres fall into the same normalised rectangle -- they all sample the same neighbourhoods) for ONE head, and
 //   1. one thread TMA-loads (cp.async.bulk.tensor.5d, tensor = [D, M, W_l, H_l, N] per level, box = [D, 1, BW_l, BH_l, 1])
@@ -96,7 +96,7 @@ struct MsdaQp {
 
 // NW warps per CTA.  KC > 0: compile-time K = L*P (PC = P).
 //
-// The kernel is ISSUE bound (r2 ncu: ~430 warp instructions per (query, head) against 64 data wavefronts), so the hot
+// The kernel is issue bound (~430 warp instructions per (query, head) against 64 data wavefronts), so the hot
 // path is written for instruction count: everything that depends only on the lane's role (its sample's level: map and
 // window geometry) lives in registers, the region's query list is a shared-memory table built once per CTA, global
 // indices are 32-bit (host-checked), the bf16 rows are unpacked with one shift / one mask per element pair, and the
@@ -464,7 +464,7 @@ extern "C" int vllm_msda_set_window_fill(int tma) {
   return VLLM_OK;
 }
 
-constexpr int WIN_FILL_DEFAULT_BF16 = (1 << MSDA_WIN_LEVELS) - 1;   // measured (profiles/r2_msda_window_sweep.json)
+constexpr int WIN_FILL_DEFAULT_BF16 = (1 << MSDA_WIN_LEVELS) - 1;   // every level staged; not re-tuned for the H100
 constexpr int WIN_FILL_DEFAULT_F32 = (1 << MSDA_WIN_LEVELS) - 1;
 
 static void set_fill(MsdaWin& wp, int vb) {
@@ -498,8 +498,8 @@ static bool build_window(WinCacheEntry& e, const ValT* value, const int64_t* hs,
     tot += H * W;
   }
   if (tot != S) return false;
-  // level-0 patch: 16 x 32 pixels for bf16 rows (64 B): 159 KB of windows, one 32-warp CTA per SM (measured best,
-  // profiles/r2_msda_window_sweep.json: the halo is amortised over 4x the queries of an 8 x 16 patch); 8 x 8 for fp32 rows
+  // level-0 patch: 16 x 32 pixels for bf16 rows (64 B): 159 KB of windows, one 32-warp CTA per SM (the halo is
+  // amortised over 4x the queries of an 8 x 16 patch; the choice has not been re-swept on the H100); 8 x 8 for fp32 rows
   // (128 B): 95 KB, two 16-warp CTAs per SM
   wp.PH = g_win_ph > 0 ? g_win_ph : (VB == 2 ? 16 : 8);
   wp.PW = g_win_pw > 0 ? g_win_pw : (VB == 2 ? 32 : 8);

@@ -1,4 +1,4 @@
-"""B200-native Grounding-DINO deformable blocks (the region/mask decoder's hot layers).
+"""H100-native Grounding-DINO deformable blocks (the region/mask decoder's hot layers).
 
 Same class names, constructor arguments, parameter names and call signatures as
 visionllmv2/model/grounding_dino/modeling_ov_grounding_dino_mask_dn.py:
@@ -11,7 +11,7 @@ visionllmv2/model/grounding_dino/modeling_ov_grounding_dino_mask_dn.py:
   GroundingDinoFusionLayer                    :1039-1102 (LN, bi-attention, LayerScale residuals)
   GroundingDinoEncoderLayer                   :1216-1289 (fusion -> text enhancer -> deformable layer)
 so reference state dicts load unchanged and the modules can be assigned over the reference classes
-(INTEGRATION.md).  Projections run on the tcgen05 GEMM (offset and weight projections share one launch),
+(INTEGRATION.md).  Projections run on the wgmma GEMM (offset and weight projections share one launch),
 LayerNorm/residuals on the row kernels, attention on the fused attention kernel, the gather on
 vllm_msda_forward_f32 -- never the grid_sample fallback the reference silently drops to (:777-779).
 Forward / inference only.
@@ -44,7 +44,7 @@ class GroundingDinoMultiscaleDeformableAttention(nn.Module):
         self._packed = None
         self._reset_parameters()
 
-    # the reference module always returns the attention weights (gd.py:784); an owner that never reads them (the B200 GDINO
+    # the reference module always returns the attention weights (gd.py:784); an owner that never reads them (the H100 GDINO
     # stage) clears this so the fused gather kernel skips the [B, Lq, M, L, P] side output
     need_weights = True
 

@@ -1,6 +1,6 @@
 """Grounding-DINO query-selection, heads and post-processing of the region/mask decoder (SURVEY 8a a12, a18, a20,
 a21), restated from visionllmv2/model/grounding_dino/modeling_ov_grounding_dino_mask_dn.py and
-visionllmv2/eval/eval_det.py.  Dense math runs on the tcgen05 GEMM; the integer work (top-k, //, %, gathers)
+visionllmv2/eval/eval_det.py.  Dense math runs on the wgmma GEMM; the integer work (top-k, //, %, gathers)
 uses the same torch primitives the reference uses so indices -- including tie order -- are identical.
 
   GroundingDinoMLPPredictionHead        gd.py:3704-3720   (bbox / mask-embed / patch2query MLPs, ReLU epilogues)

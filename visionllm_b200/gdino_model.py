@@ -7,7 +7,7 @@ What runs where:
   backbone (a13)            HF `AutoBackbone` (Swin) exactly as the reference builds it (:471-504) -- third-party
                             torch code on the GPU, or `visionllm_b200.swin.B200SwinBackbone` (same state dict) when
                             passed in.  Everything after it is ours.
-  neck (a14)                1x1 / 3x3-stride-2 projections as tcgen05 GEMMs over channels-last rows + the GroupNorm
+  neck (a14)                1x1 / 3x3-stride-2 projections as wgmma GEMMs over channels-last rows + the GroupNorm
                             kernel (csrc/groupnorm.cu); sine position embedding, masks, `spatial_shapes`,
                             `level_start_index`, `valid_ratios` with the reference's own integer / fp32 arithmetic.
   encoder / decoder         visionllm_b200.gdino layers (MSDA kernel, fused attention, GEMM epilogues).

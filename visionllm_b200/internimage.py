@@ -1,4 +1,4 @@
-"""B200-native InternImage backbone (SURVEY.md 8a-a13, second option: InternImage-H for the Grounding-DINO stage).
+"""H100-native InternImage backbone (SURVEY.md 8a-a13, second option: InternImage-H for the Grounding-DINO stage).
 
 Drop-in for the reference classes `InternImage` / `build_internimage_h` / `GroundingDinoInternImageBackbone`
 (visionllmv2/model/grounding_dino/modeling_ov_grounding_dino_mask_dn.py:4689-5209) and the `DCNv3` module they are
@@ -8,7 +8,7 @@ norm in an `nn.Sequential` of layout permutes, so the LayerNorms live under `...
 forward contract (`forward(x[B,3,H,W]) -> [level maps]`).
 
 Execution on our kernels, channels-last throughout (the reference permutes to NCHW and back around every conv):
-  stem / downsample 3x3-s2 convs   tap-gather + tcgen05 GEMM (+bias)                     ops.linear
+  stem / downsample 3x3-s2 convs   tap-gather + wgmma GEMM (+bias)                     ops.linear
   LayerNorms                       row kernel; the `LN -> GELU` tail of the depthwise branch in ONE pass
   depthwise 5x5 (3x3) conv         csrc/dwconv.cu (register-tiled, NHWC)                  ops.dwconv_nhwc
   input_proj                       GEMM -> fp32 (the core op is fp32, dcnv3.py:331-340)
@@ -301,7 +301,7 @@ class InternImageBlock(nn.Module):
 
 class B200InternImage(nn.Module):
     """`InternImage` (gd.py:4978-5152).  forward(x[B,3,H,W]) -> list of level maps.  `channels_last_out=True` (default
-    inside the B200 GDINO stage) returns [B, h, w, C] maps flagged `_b200_nhwc`; False returns the reference's
+    inside the H100 GDINO stage) returns [B, h, w, C] maps flagged `_b200_nhwc`; False returns the reference's
     contiguous NCHW maps."""
 
     def __init__(self, core_op="DCNv3", channels=64, depths=(3, 4, 18, 5), groups=(3, 6, 12, 24), mlp_ratio=4.,

@@ -1,4 +1,4 @@
-"""B200-native InternLM2 decoder (the 26B preset's LLM): drop-in for the vendored
+"""H100-native InternLM2 decoder (the 26B preset's LLM): drop-in for the vendored
 visionllmv2/model/internlm2/modeling_internlm2.py `InternLM2ForCausalLM` as the reference calls it
 (modeling_visionllmv2.py:724-736: `self.llm(inputs_embeds=..., output_hidden_states=True)`, logits through
 `self.llm.output`).  State-dict names are the reference's: model.tok_embeddings, model.layers.N.attention.{wqkv,wo},

@@ -1,4 +1,4 @@
-"""B200-native InternViT: drop-in for the reference ``InternVisionModel``.
+"""H100-native InternViT: drop-in for the reference ``InternVisionModel``.
 
 Mirrors visionllmv2/model/internvit/modeling_intern_vit.py (class/attribute/state-dict
 names identical, so reference checkpoints load with ``load_state_dict``):

@@ -1,4 +1,4 @@
-"""B200-native Llama decoder (Vicuna-7B): drop-in for HF ``LlamaForCausalLM`` as the reference uses it
+"""H100-native Llama decoder (Vicuna-7B): drop-in for HF ``LlamaForCausalLM`` as the reference uses it
 (visionllmv2/model/modeling_visionllmv2.py:143,420,724-738: inputs_embeds in, hidden_states[-1] and
 fp32 logits out; RMSNorm := apex FusedRMSNorm via visionllmv2/train/llama_forward_monkey_patch.py:168-180).
 

@@ -1,6 +1,6 @@
 """Composite forward: B200 drop-in for ``VisionLLMv2Model.forward`` on the perception / chat eval path.
 
-Restates visionllmv2/model/modeling_visionllmv2.py (paths relative to /root/reference/VisionLLMv2/):
+Restates visionllmv2/model/modeling_visionllmv2.py (paths relative to the VisionLLMv2/ directory of the reference):
   :119-198  constructor-injected sub-models (vis_encoder, llm, gdino) and the vl_bridge variants
   :381-392  pixel_shuffle (space-to-depth x2)
   :419-527  [EMB] super-link injection after tool tokens (overwrite form used by train/eval batches)
@@ -46,7 +46,7 @@ class VisionLLMv2ModelOutput(ModelOutput):
 
 
 class BridgeLinear(nn.Linear):
-    """nn.Linear whose forward is the tcgen05 GEMM (optionally with a fused activation)."""
+    """nn.Linear whose forward is the wgmma GEMM (optionally with a fused activation)."""
 
     def forward(self, x, act=None):
         return ops.linear(x, self.weight, bias=self.bias, act=act)

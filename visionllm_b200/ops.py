@@ -59,7 +59,7 @@ def linear(x, weight, bias=None, act=None, colscale=None, residual=None, out_dty
     """y = epi(x @ weight.T): x [..., K] bf16, weight [N, K] bf16 (nn.Linear layout).
 
     epi = (+bias) -> act -> (*colscale) -> (+residual); act='swiglu' expects gate/up rows
-    interleaved in `weight` and returns N/2 columns.  One tcgen05 kernel launch.
+    interleaved in `weight` and returns N/2 columns.  One wgmma kernel launch.
     row_keep: optional bool/uint8 [...] (one per row): rows with False are stored as exact zeros
     (`masked_fill(~row_keep[..., None], 0)` folded into the epilogue).
     """
@@ -111,7 +111,7 @@ def linear(x, weight, bias=None, act=None, colscale=None, residual=None, out_dty
 
 
 def gemm_tn(a, b, a_mn=False, b_mn=False, out_dtype=torch.bfloat16):
-    """C[M, N] = sum_k A(m, k) B(n, k) on the tcgen05 GEMM with K-major or MN-major operands (the backward GEMMs):
+    """C[M, N] = sum_k A(m, k) B(n, k) on the wgmma GEMM with K-major or MN-major operands (the backward GEMMs):
     a is [M, K] (a_mn=False) or [K, M] (a_mn=True), b is [N, K] or [K, N]; 2-D bf16, unit inner stride.
       dgrad: gemm_tn(dy, W, b_mn=True)            -> dx [T, in]
       wgrad: gemm_tn(dy, x, a_mn=True, b_mn=True) -> dW [out, in]"""

@@ -1,4 +1,4 @@
-"""B200-native region encoder (SURVEY.md 8f rank 4): drop-in for `RegionEncoder`
+"""H100-native region encoder (SURVEY.md 8f rank 4): drop-in for `RegionEncoder`
 (visionllmv2/model/region_encoder.py:66-145; built at modeling_visionllmv2.py:247-252 with mask_pool_type='grid_sample',
 called at :687 with the [n_regions, 3, H, W] images, the [n_regions, 1, H, W] 0/1 region masks and the last three ViT
 hidden states).  Same constructor, parameter names (`mask_embedding.{0,1,3,4,6}`, `up_dim`, `region_query`,

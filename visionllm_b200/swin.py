@@ -1,4 +1,4 @@
-"""Swin Transformer backbone of the Grounding-DINO stage (SURVEY 8a row a13) on the B200 kernels.
+"""Swin Transformer backbone of the Grounding-DINO stage (SURVEY 8a row a13) on the H100 kernels.
 
 The reference builds it with HF `AutoBackbone.from_config(config.backbone_config)`
 (grounding_dino/modeling_ov_grounding_dino_mask_dn.py:471-504) -- third-party `transformers.models.swin.modeling_swin`

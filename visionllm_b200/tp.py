@@ -320,8 +320,7 @@ class TPLlamaForCausalLM(nn.Module):
         self.theta = theta
         self.shards = None
         # forward_pipelined: optional SM budgets of the compute GEMMs / of the scatter GEMM (0 = all SMs, the default).
-        # Measured on 8 x B200 (DESIGN 8): every budget tried LOSES against plain two-stream overlap (45.7 ms) -- the
-        # scatter GEMM's peer stores need many SMs to fill the links (28 SMs: 57.6 ms, 16 SMs: 71.0 ms)
+        # Not measured on H100s: the scatter GEMM's peer stores need many SMs to fill the links, so a budget may lose.
         self.compute_sms, self.scatter_sms = 0, 0
         if shards is not None:
             self.load_shards(shards, device, dtype)

@@ -8,7 +8,7 @@ Megatron split of the decoder layer over the ranks of a torch.distributed group:
   replicated       the residual stream, both RMSNorms, the final norm and the lm_head (every rank holds all token rows)
 The backward mirrors it through two tiny autograd Functions: `CopyToTP` (identity forward, all-reduce of the input
 gradient backward) in front of the column-parallel GEMMs and `ReduceFromTP` (all-reduce forward, identity backward)
-behind the row-parallel ones.  Every compute op in between is a kernel of this repo (train.py's Functions: tcgen05 GEMMs
+behind the row-parallel ones.  Every compute op in between is a kernel of this repo (train.py's Functions: wgmma GEMMs
 with MN-major dgrad / wgrad, batched attention backward, RMSNorm / SwiGLU / RoPE / CE kernels); the collectives are NCCL
 calls -- the peer-memory fusion of tp.py's forward exchange is not extended to the backward (DESIGN 10).
 

@@ -6,11 +6,11 @@ IGNORE_INDEX; labels of the [EMB] slots are ignored).  Here every op of the deco
 whose forward AND backward are this repo's kernels:
 
   op                forward                                   backward
-  Linear            tcgen05 GEMM (ops.linear)                 dgrad / wgrad on the same kernel with MN-major operands
+  Linear            wgmma GEMM (ops.linear)                 dgrad / wgrad on the same kernel with MN-major operands
                                                               (ops.gemm_tn: no transposed copies of W, dy or x)
   RMSNorm           vllm_rmsnorm_bf16                         vllm_rmsnorm_bwd_bf16 (dx + fp32 dweight)
   RoPE              vllm_rope_bf16 (q and k heads)            the same kernel with -sin (the rotation's transpose)
-  causal attention  tcgen05 flash forward (ops.attention)     materialised backward: 5 block-diagonal batched tcgen05 GEMMs
+  causal attention  wgmma flash forward (ops.attention)     materialised backward: 5 block-diagonal batched wgmma GEMMs
                                                               over all (batch, head) matrices of the layer with causal
                                                               tile / K-range skipping + two row kernels (softmax recompute,
                                                               softmax backward); scores / probabilities in bf16 like HF's
@@ -83,7 +83,7 @@ def head_stack(t, B, T, parts, H, D, to_stacked):
 
 
 def gemm_batched(a, b, n_batch, M, N, K, a_mn=False, b_mn=False, causal=0, out_dtype=torch.bfloat16, out=None):
-    """n_batch block-diagonal products C_b = A_b . B_b^T in one tcgen05 launch (operands / output stacked along rows)."""
+    """n_batch block-diagonal products C_b = A_b . B_b^T in one wgmma launch (operands / output stacked along rows)."""
     if out is None:
         out = torch.empty((n_batch * M, N), dtype=out_dtype, device=a.device)
     with torch.cuda.device(a.device), ops._Prof("gemm", 2.0 * n_batch * M * N * K * (0.5 if causal else 1.0), 0.0,
@@ -155,7 +155,7 @@ class LinearFn(torch.autograd.Function):
             dy2 = padded[:, :dy.shape[-1]]
         x2 = x.reshape(-1, x.shape[-1])
         dx = ops.gemm_tn(dy2, w, b_mn=True).view(x.shape) if ctx.needs_input_grad[0] else None
-        # wgrad: fp32 accumulation in TMEM, ONE rounding to the parameter dtype in the epilogue (== fp32 result .to(bf16))
+        # wgrad: fp32 accumulation in registers, ONE rounding to the parameter dtype in the epilogue (== fp32 result .to(bf16))
         dw = None
         if ctx.needs_input_grad[1]:
             dw = ops.gemm_tn(dy2, x2, a_mn=True, b_mn=True, out_dtype=torch.bfloat16 if w.dtype == torch.bfloat16 else torch.float32)

@@ -1,4 +1,4 @@
-"""B200-native UniPose deformable layers (SURVEY.md 8f rank 4): drop-ins for
+"""H100-native UniPose deformable layers (SURVEY.md 8f rank 4): drop-ins for
 `MSDeformAttn` (visionllmv2/model/unipose/ops/modules/ms_deform_attn.py:33-158),
 `DeformableTransformerEncoderLayer` and `DeformableTransformerDecoderLayer`
 (visionllmv2/model/unipose/modeling_unipose.py:3132-3186, 3188-3323) -- the consumers of the MSDA operator in the
@@ -374,7 +374,7 @@ class BiMultiHeadAttention(nn.Module):
     """modeling_unipose.py:1943-2082 (parameter names v_proj / l_proj / values_v_proj / values_l_proj / out_v_proj /
     out_l_proj).  Both directions share S = (v_proj(v) * scale) l_proj(l)^T: softmax over the text keys updates the image
     tokens, softmax over the image keys of S^T the text tokens; the reference's global `S - S.max()` and +-50000 clamps do not
-    change either softmax.  Masks: True = padding.  Two tcgen05 attention calls (head_dim = embed_dim / heads, 256 for the
+    change either softmax.  Masks: True = padding.  Two wgmma attention calls (head_dim = embed_dim / heads, 256 for the
     released config) on packed projection GEMMs."""
 
     def __init__(self, v_dim, l_dim, embed_dim, num_heads, dropout=0.1, cfg=None):

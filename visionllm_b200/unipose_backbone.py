@@ -1,4 +1,4 @@
-"""UniPose's image backbone on the B200 kernels: the reference's own `SwinTransformer` + `Joiner`
+"""UniPose's image backbone on the H100 kernels: the reference's own `SwinTransformer` + `Joiner`
 (unipose/modeling_unipose.py:1212-1226 Joiner, :1277-1355 WindowAttention, :1357-1454 SwinTransformerBlock,
 :1456-1494 PatchMerging, :1496-1595 BasicLayer, :1597-1636 PatchEmbed, :1638-1858 SwinTransformer, :4082-4120 / :4162-4222
 builders), inference path.
