@@ -217,55 +217,6 @@ class MsdaEncoderBf16Workload(MsdaEncoderWorkload):
         return c
 
 
-class MsdaEncoderPairsWorkload(MsdaEncoderBf16Workload):
-    """cfg 2b fast mode on the paired-row layout: a step = `ms_deform_attn_pack_pairs` (bf16 value -> [N,S,M,2,32], one
-    HBM pass) + `ms_deform_attn_forward_pairs` (two 128-byte line fetches per sample instead of four); both launches
-    are inside the timed region, the algorithmic bytes stay those of the bf16 operator (the pair tensor is internal)."""
-    metric = "msda_encoder_layer_images_per_sec_bf16_value"
-
-    def _run(self, value, loc, attw):
-        pairs = self.ext.ms_deform_attn_pack_pairs(value, self.shapes, self.lsi)
-        return self.ext.ms_deform_attn_forward_pairs(pairs, self.shapes, self.lsi, loc, attw)
-
-    def step_device(self):
-        self.out = self._run(self.value, self.loc, self.attw)
-
-    def step_e2e(self):
-        for d, h in zip(self.d_in, self.h_in):
-            d.copy_(h, non_blocking=True)
-        self.h_out.copy_(self._run(*self.d_in), non_blocking=True)
-
-    def dominant_kernel_ms(self, steps):
-        torch = self.torch
-        pairs = self.ext.ms_deform_attn_pack_pairs(self.value, self.shapes, self.lsi)
-        torch.cuda.synchronize()
-        evs = []
-        for _ in range(steps):
-            e0, e1, e2 = (torch.cuda.Event(enable_timing=True) for _ in range(3))
-            pairs = None                       # hand the block back first: no cudaMalloc inside the timed interval
-            e0.record()
-            pairs = self.ext.ms_deform_attn_pack_pairs(self.value, self.shapes, self.lsi)
-            e1.record()
-            self.ext.ms_deform_attn_forward_pairs(pairs, self.shapes, self.lsi, self.loc, self.attw)
-            e2.record()
-            evs.append((e0, e1, e2))
-        torch.cuda.synchronize()
-        self.pack_ms = sum(a.elapsed_time(b) for a, b, _ in evs) / steps
-        self.gather_ms = sum(b.elapsed_time(c) for _, b, c in evs) / steps
-        return self.pack_ms + self.gather_ms
-
-    def roofline(self, kern_ms, peaks):
-        r = super().roofline(kern_ms, peaks)
-        r["kernel"] = "msda_pack_pairs_kernel + msda_fwd_pair_kernel (both launches of the step)"
-        r["pack_ms"], r["gather_ms"] = self.pack_ms, self.gather_ms
-        return r
-
-    def config(self):
-        c = super().config()
-        c["workload"] += ", paired-row layout (pack + gather)"
-        return c
-
-
 def anyres_tiles_1024(torch, n_pairs, device, seed, tile=448, dtype=None, tiles=5):
     """What the reference's data pipeline hands to forward() for a 1024x1024 image under 'anyres'
     (mm_utils.py:39-75: image_size 448, max 6 tiles -> (2,2) grid + thumbnail = 5 tiles): a list of
@@ -1454,7 +1405,7 @@ def tp_train_extra(rank, world, device, steps=5, warmup=2):
 
 
 WORKLOADS = {"msda_encoder": MsdaEncoderWorkload, "msda_encoder_bf16": MsdaEncoderBf16Workload,
-             "msda_encoder_pairs": MsdaEncoderPairsWorkload, "pair_forward": PairForwardWorkload, "gdino_head": GdinoHeadWorkload,
+             "pair_forward": PairForwardWorkload, "gdino_head": GdinoHeadWorkload,
              "gdino_stage": GdinoStageWorkload, "pair_forward_gdino": PairForwardGdinoWorkload,
              "llm_tp": LlmTpWorkload, "llm_tp_plain": LlmTpPlainWorkload, "internimage_h": InternImageHWorkload, "cfg1_forward": Cfg1Workload,
              "llm_train": LlmTrainWorkload, "llm_tp_train": LlmTpTrainWorkload,
@@ -1468,7 +1419,7 @@ DEFAULT_WORKLOAD = "pair_forward"
 H100_80GB_PEAK_GB = {"pair_forward": 65.3, "pair_forward_gdino": 52.4, "pair_forward_1tile": 47.5, "pair_forward_clip7b": 43.0,
                      "pair_forward_clip7b_1tile": 27.4, "llm_train": 55.5, "llm_tp_train": 47.3, "llm_tp": 20.1,
                      "llm_tp_plain": 20.1, "internimage_h": 4.6, "gdino_stage": 3.3, "gdino_head": 1.9, "unipose_stage": 2.9,
-                     "cfg1_forward": 0.3, "msda_encoder": 1.2, "msda_encoder_bf16": 1.1, "msda_encoder_pairs": 1.1}
+                     "cfg1_forward": 0.3, "msda_encoder": 1.2, "msda_encoder_bf16": 1.1}
 
 
 # --------------------------------------------------------------------------------------
@@ -1727,7 +1678,7 @@ def _cpu_llm_train(steps, warmup):
             "ms_per_step": 4 * 32 * tl * 1e3, "sample_ms_per_step": tl * 1e3, "extrapolated": True}
 
 
-_CPU = {"msda_encoder": _cpu_msda_encoder, "msda_encoder_bf16": _cpu_msda_encoder, "msda_encoder_pairs": _cpu_msda_encoder, "pair_forward": _cpu_pair_forward, "gdino_head": _cpu_msda_encoder,
+_CPU = {"msda_encoder": _cpu_msda_encoder, "msda_encoder_bf16": _cpu_msda_encoder, "pair_forward": _cpu_pair_forward, "gdino_head": _cpu_msda_encoder,
         "gdino_stage": _cpu_msda_encoder,
         "pair_forward_gdino": _cpu_pair_forward, "llm_tp": _cpu_llm_tp, "llm_tp_plain": _cpu_llm_tp, "internimage_h": _cpu_internimage_h, "cfg1_forward": _cpu_cfg1, "llm_train": _cpu_llm_train,
         "llm_tp_train": _cpu_llm_train,

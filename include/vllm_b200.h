@@ -61,19 +61,6 @@ int vllm_msda_forward_bf16v(const void* value, const int64_t* spatial_shapes, co
                             const float* sampling_loc, const float* attn_weight, void* out, int out_bf16, int batch,
                             int spatial_size, int num_heads, int channels, int num_levels, int num_query,
                             int num_point, const int64_t* host_shapes_hint, void* stream);
-/* Paired-row fast mode: the gather is bound by L1 line fetches, not bytes -- four corner rows = four 128-byte lines
- * in the reference layout.  vllm_msda_pack_pairs_bf16 rewrites a bf16 value [N,S,M,32] into pairs [N*S*M + 1, 2, 32]
- * (slot 1 = the pixel to the right inside the same image row, else 0; one extra all-zero 128-byte line at the end
- * is where corners outside the map are read from; shapes / level starts read on the device); vllm_msda_forward_pairs then fetches two lines per sample.  Same arithmetic per corner as
- * vllm_msda_forward_bf16v (fp32 products and accumulation); num_levels*num_point even and <= 32, channels == 32,
- * pairs 128-byte aligned. */
-int vllm_msda_pack_pairs_bf16(const void* value, void* pairs, const int64_t* spatial_shapes,
-                              const int64_t* level_start_index, int batch, int spatial_size, int num_heads,
-                              int channels, int num_levels, void* stream);
-int vllm_msda_forward_pairs(const void* pairs, const int64_t* spatial_shapes, const int64_t* level_start_index,
-                            const float* sampling_loc, const float* attn_weight, void* out, int out_bf16, int batch,
-                            int spatial_size, int num_heads, int channels, int num_levels, int num_query,
-                            int num_point, const int64_t* host_shapes_hint, void* stream);
 /* fp64 instance of the same operator (AT_DISPATCH_FLOATING_TYPES,
  * ms_deform_attn_cuda.cu:258); always the strict kernel. */
 int vllm_msda_forward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
@@ -101,16 +88,27 @@ int vllm_msda_backward_f64(const double* value, const int64_t* spatial_shapes, c
  * h_low/w_low are 0 when bit0 is clear. */
 int vllm_msda_sample_indices_f32(const int64_t* spatial_shapes, const float* sampling_loc, int32_t* out_hwm,
                                  long long n_samples, int num_levels, int num_point, void* stream);
-/* Tuning knob for bench sweeps (process-global, not part of the drop-in API): 0 default; 1-4 tile shapes of the fp32
- * warp-gather kernel. */
+/* Path selection for tests and benchmarks (process-global, not part of the drop-in API).  Every value forces a path
+ * the library also takes by itself on other inputs, so a test can compare two paths on one input:
+ *   VLLM_MSDA_DEFAULT         the dispatch described here
+ *   VLLM_MSDA_NO_HINT         vllm_msda_forward_f32 ignores host_shapes_hint (linear query tiles instead of 2-D pixel
+ *                             patches: what a caller that passes NULL gets)
+ *   VLLM_MSDA_BF16_NO_WINDOW  vllm_msda_forward_bf16v skips the window kernel and runs the warp-gather kernel, as it does
+ *                             for shapes the window kernel does not cover
+ *   VLLM_MSDA_FP32_WINDOW     vllm_msda_forward_f32 (non-strict) tries the window kernel first
+ * Any other value: VLLM_EINVAL, nothing changes. */
+#define VLLM_MSDA_DEFAULT 0
+#define VLLM_MSDA_NO_HINT 4
+#define VLLM_MSDA_BF16_NO_WINDOW 32
+#define VLLM_MSDA_FP32_WINDOW 33
 int vllm_msda_set_variant(int variant);
-/* Encoder shape (num_query == spatial_size, host_shapes_hint given, <= 4 levels, channels == 32): vllm_msda_forward_f32
- * (non-strict) and vllm_msda_forward_bf16v run the TMA-staged window kernel (csrc/msda_win.cu): one CTA per (image
- * region, head) loads the bounded value window of every level into shared memory with cp.async.bulk.tensor (zero fill
- * outside the map = the operator's zero padding) and gathers from there; a (query, head) with a sample outside its
- * window falls back to the global-memory path inside the same kernel (bit-identical sums).  Variant 32 disables the
- * window path for bf16 values, variants 1-4 for fp32.  vllm_msda_set_window: tuning knob (process-global) -- level-0
- * patch height / width in pixels and level-0 halo; 0 = default (8 x 16, halo 8 for bf16 rows; 8 x 8, halo 6 for fp32). */
+/* Encoder shape (num_query == spatial_size, host_shapes_hint given, <= 4 levels, channels == 32): vllm_msda_forward_bf16v
+ * -- and vllm_msda_forward_f32 (non-strict) under VLLM_MSDA_FP32_WINDOW -- run the TMA-staged window kernel
+ * (csrc/msda_win.cu): one CTA per (image region, head) loads the bounded value window of every level into shared memory
+ * with cp.async.bulk.tensor (zero fill outside the map = the operator's zero padding) and gathers from there; a (query,
+ * head) with a sample outside its window falls back to the global-memory path inside the same kernel (bit-identical
+ * sums).  vllm_msda_set_window: tuning knob (process-global) -- level-0 patch height / width in pixels and level-0 halo;
+ * 0 = default (16 x 32, halo 8 for bf16 rows; 8 x 8, halo 6 for fp32). */
 int vllm_msda_set_window(int patch_h, int patch_w, int halo0);
 /* Window fill of the encoder kernel: bit l of `tma` set = level l's window arrives as one TMA box (cp.async.bulk.tensor.5d),
  * clear = cooperative cp.async (one 64 / 128-byte row per thread and step); 1 = every level by TMA (its r2 meaning),
@@ -185,8 +183,6 @@ int vllm_gemm_bf16_rowmask(const void* A, int lda, const void* B, int ldb, void*
  * scatter GEMM alone.  A GEMM CTA owns its SM, so the link-bound exchange kernels of another stream (tensor-parallel
  * micro-batches, visionllm_b200/tp.py) overlap a GEMM only on SMs its grid leaves free. */
 int vllm_gemm_set_sm_limit(int all_gemms, int scatter_gemm);
-/* Tuning knob (process-global): 0 = auto (default: 128x128 tiles; the scatter GEMM always uses
- * 128x256), 1 = 128x128 tiles, 2 = 128x256 tiles. */
 /* Stride-1 KxK convolution over a zero-padded channels-last map as ONE implicit GEMM (no im2col buffer): the 3x3
  * `output_convs` of the Grounding-DINO mask-feature FPN (modeling_ov_grounding_dino_mask_dn.py:2136-2146, :2476).
  * xpad: [pad_pixels, channels] bf16 = the padded images flattened (image rows of `padded_width` pixels, images back
@@ -198,9 +194,11 @@ int vllm_gemm_set_sm_limit(int all_gemms, int scatter_gemm);
 int vllm_conv_rows_bf16(const void* xpad, long long pad_pixels, int channels, int padded_width, int kernel_h,
                         int kernel_w, const void* weight, int ldw, void* out, int ldo, int out_channels,
                         const void* bias, int act, void* stream);
+/* Tile selection for tests and sweeps (process-global): VLLM_GEMM_DEFAULT = 128 x 128 tiles, VLLM_GEMM_WIDE_TILE =
+ * 128 x 256 tiles, which the scatter GEMM always uses.  Any other value: VLLM_EINVAL, nothing changes. */
+#define VLLM_GEMM_DEFAULT 0
+#define VLLM_GEMM_WIDE_TILE 2
 int vllm_gemm_set_variant(int variant);
-/* Tuning knob: force the tile-rasterisation group size (row-blocks per group); 0 = heuristic. */
-int vllm_gemm_set_group_m(int group_m);
 
 /* ---- row-wise norms and RoPE (bf16 in/out, fp32 statistics) ----------------------
  * vllm_rmsnorm_bf16 replaces apex.normalization.FusedRMSNorm forward
@@ -251,12 +249,10 @@ int vllm_dwconv_nhwc_bf16(const void* x, const void* weight_taps, const void* bi
  * channels/groups % 8 == 0, channels <= 2048.  workspace: vllm_groupnorm_workspace_bytes(batch, groups) bytes of
  * device memory (per-chunk partial sums; combined in a fixed order, so results are run-to-run identical). */
 long long vllm_groupnorm_workspace_bytes(int batch, int groups);
-int vllm_groupnorm_nhwc_bf16(const void* x, void* y, const void* gamma, const void* beta, int batch, long long hw,
-                             int channels, int groups, float eps, int relu, void* workspace, long long workspace_bytes,
-                             void* stream);
-/* The same over the valid [h, w] corner of a padded grid: pixel (r, c) of image n is read at pixel index
- * n * x_image_pitch + r * x_w_pitch + c (what vllm_conv_rows_bf16 leaves for a 3x3 convolution); y is the contiguous
- * [batch, h * w, channels] result.  Same statistics order, so the result equals copying the corner out first. */
+/* x is the valid [h, w] corner of a possibly padded grid: pixel (r, c) of image n is read at pixel index
+ * n * x_image_pitch + r * x_w_pitch + c (what vllm_conv_rows_bf16 leaves for a 3x3 convolution; a contiguous
+ * [batch, hw, channels] input is h = 1, w = x_w_pitch = x_image_pitch = hw); y is the contiguous [batch, h * w, channels]
+ * result.  The statistics order does not depend on the pitches, so the result equals copying the corner out first. */
 int vllm_groupnorm_nhwc_bf16_grid(const void* x, void* y, const void* gamma, const void* beta, int batch, long long h, long long w,
                                   long long x_w_pitch, long long x_image_pitch, int channels, int groups, float eps, int relu,
                                   void* workspace, long long workspace_bytes, void* stream);
@@ -264,10 +260,8 @@ int vllm_groupnorm_nhwc_bf16_grid(const void* x, void* y, const void* gamma, con
  * out = lateral + F.interpolate(top, size=(out_h, out_w), mode="bilinear", align_corners=False) over channels-last bf16
  * maps top [batch, in_h, in_w, channels], lateral / out [batch, out_h, out_w, channels] in one pass (ATen's
  * upsample_bilinear2d arithmetic; the interpolated value is rounded to bf16 before the bf16 add, like the torch ops).
- * channels % 8 == 0. */
-int vllm_upsample_add_nhwc_bf16(const void* top, const void* lateral, void* out, int batch, int in_h, int in_w, int out_h,
-                                int out_w, int channels, void* stream);
-/* _ex: `top` images top_image_pitch elements apart (a level slab of the flattened encoder output, read in place);
+ * channels % 8 == 0.  `top` images lie top_image_pitch elements apart (a level slab of the flattened encoder output, read
+ * in place; in_h * in_w * channels for a contiguous tensor);
  * out_pad > 0 writes the result into the interior of a caller-zeroed [batch, out_h + 2 pad, out_w + 2 pad, channels] map --
  * the zero-padded input of the 3x3 output convolution that follows (:2493), without a pad copy. */
 int vllm_upsample_add_nhwc_bf16_ex(const void* top, long long top_image_pitch, const void* lateral, void* out, int batch, int in_h,

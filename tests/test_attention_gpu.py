@@ -30,9 +30,8 @@ def ref_attn(q, k, v, causal, seqlens=None):
 def variant(request):
     """Run every case on the wgmma kernel (head_dim 128 / 256) and on the warp-MMA kernel."""
     from visionllm_b200 import _lib
-    _lib.lib().vllm_attention_set_variant(request.param)
-    yield request.param
-    _lib.lib().vllm_attention_set_variant(0)
+    with _lib.knob("attention_set_variant", request.param):
+        yield request.param
 
 
 def check(out, ref):
@@ -179,11 +178,8 @@ def test_attention_wgmma_key_mask_and_split_kv(D, Tq, Tk):
             s_ = s_.masked_fill(~mask[:, None, None, :], float("-inf"))
         ref = (torch.softmax(s_, -1) @ v.float().permute(0, 2, 1, 3)).permute(0, 2, 1, 3).reshape(B, Tq, H * D)
         check(out, ref)
-        _lib.lib().vllm_attention_set_variant(1)
-        try:
+        with _lib.knob("attention_set_variant", 1):
             warp = ops.attention(q, k, v, key_mask=mask)
-        finally:
-            _lib.lib().vllm_attention_set_variant(0)
         check(out, warp.float())
 
 

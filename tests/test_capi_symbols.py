@@ -5,6 +5,8 @@ import glob
 import os
 import re
 
+import pytest
+
 from visionllm_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -31,6 +33,10 @@ def test_library_exports_every_declared_symbol():
 
 def test_python_binding_covers_the_header():
     assert set(declared_symbols()) == set(_lib.exported_symbols())
+    # the named knob values are the header's
+    src = open(os.path.join(ROOT, "include", "vllm_b200.h")).read()
+    defines = {k: int(v) for k, v in re.findall(r"#define VLLM_((?:MSDA|GEMM)_[A-Z0-9_]+) (\d+)", src) if k != "MSDA_STRICT"}
+    assert defines and defines == {k: getattr(_lib, k) for k in dir(_lib) if k.startswith(("MSDA_", "GEMM_"))}
 
 
 def test_version_string():
@@ -42,6 +48,11 @@ def test_round2_entry_points_marshal_and_accept_empty_problems():
     with a malformed one (negative error code): checks the Python-side signatures against the library without a GPU."""
     L = _lib.lib()
     assert L.vllm_msda_set_window(0, 0, 0) == 0 and L.vllm_msda_set_window(-1, 0, 0) < 0
+    assert L.vllm_msda_set_variant(_lib.MSDA_DEFAULT) == 0 and L.vllm_msda_set_variant(1) < 0      # not a named value
+    assert L.vllm_gemm_set_variant(_lib.GEMM_DEFAULT) == 0 and L.vllm_gemm_set_variant(1) < 0
+    with pytest.raises(_lib.VllmB200Error):                                                          # a rejected value must not
+        with _lib.knob("msda_set_variant", 1):                                                       # silently test the default path
+            pass
     assert L.vllm_det_postprocess_f32(None, None, None, 0, 100, 80, 256, 100, None, None, None, None, None, None) == 0
     assert L.vllm_det_postprocess_f32(None, None, None, 1, 100, 80, 40, 100, None, None, None, None, None, None) < 0   # ld < K
     assert L.vllm_mask_postprocess_f32(None, None, 0, 64, 64, 4, 250, 250, 480, 500, None, None) == 0

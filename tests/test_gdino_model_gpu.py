@@ -140,7 +140,7 @@ def test_groupnorm_kernel(shape, relu):
 
 @pytest.mark.parametrize("shape", [(2, 16, 16, 32, 32, 256), (1, 13, 17, 25, 34, 64), (2, 8, 8, 8, 8, 48), (1, 5, 7, 20, 9, 8)])
 def test_upsample_add_kernel_matches_the_torch_ops(shape):
-    """vllm_upsample_add_nhwc_bf16 (FPN top-down step) vs the reference's ops: bf16 F.interpolate(bilinear,
+    """vllm_upsample_add_nhwc_bf16_ex (FPN top-down step) vs the reference's ops: bf16 F.interpolate(bilinear,
     align_corners=False) + bf16 add.  ATen's kernel may contract the tap sums differently, so the interpolated value can
     differ by a bf16 ulp: checked against the fp32 interpolation with one bf16 rounding of each step."""
     from visionllm_b200 import ops

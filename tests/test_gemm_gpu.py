@@ -12,8 +12,12 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-# tile-width variants under test (bring-up: VLLM_TEST_GEMM_VARIANTS=1 isolates the 128-column tile)
-VARIANTS = [int(v) for v in os.environ.get("VLLM_TEST_GEMM_VARIANTS", "1,2").split(",")]
+from visionllm_b200 import _lib  # noqa: E402
+
+# tile widths under test, named by their width in 128-column units (bring-up: VLLM_TEST_GEMM_VARIANTS=1 isolates the
+# 128-column tile)
+TILES = {"1": _lib.GEMM_DEFAULT, "2": _lib.GEMM_WIDE_TILE}
+VARIANTS = [pytest.param(TILES[t], id=t) for t in os.environ.get("VLLM_TEST_GEMM_VARIANTS", "1,2").split(",")]
 
 
 def ops():
@@ -43,14 +47,10 @@ SHAPES = [(128, 256, 64), (128, 256, 128), (256, 512, 256), (1025, 3200, 3200), 
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("M,N,K", SHAPES)
 def test_gemm_plain(M, N, K, variant):
-    from visionllm_b200 import _lib
     x, w = mk(M, N, K)
-    _lib.lib().vllm_gemm_set_variant(variant)
-    try:
+    with _lib.knob("gemm_set_variant", variant):
         out = ops().linear(x, w)
         torch.cuda.synchronize()
-    finally:
-        _lib.lib().vllm_gemm_set_variant(0)
     ref = x.float() @ w.float().T
     close(out, ref)
 
@@ -58,19 +58,15 @@ def test_gemm_plain(M, N, K, variant):
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("act", ["gelu", "relu", "silu", "quick_gelu", None])
 def test_gemm_epilogues(act, variant):
-    from visionllm_b200 import _lib
     M, N, K = 520, 768, 320
     x, w = mk(M, N, K, seed=3)
     g = torch.Generator(device="cuda").manual_seed(9)
     bias = torch.randn(N, device="cuda", generator=g).bfloat16()
     ls = (torch.rand(N, device="cuda", generator=g) * 0.2).bfloat16()
     res = torch.randn(M, N, device="cuda", generator=g).bfloat16()
-    _lib.lib().vllm_gemm_set_variant(variant)
-    try:
+    with _lib.knob("gemm_set_variant", variant):
         out = ops().linear(x, w, bias=bias, act=act, colscale=ls, residual=res)
         out32 = ops().linear(x, w, bias=bias, act=act, out_dtype=torch.float32)
-    finally:
-        _lib.lib().vllm_gemm_set_variant(0)
     y = x.float() @ w.float().T + bias.float()
     if act == "gelu":
         y = torch.nn.functional.gelu(y)
@@ -87,18 +83,14 @@ def test_gemm_epilogues(act, variant):
 
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_gemm_swiglu_interleaved(variant):
-    from visionllm_b200 import _lib
     M, I, K = 300, 1376, 512
     g = torch.Generator(device="cuda").manual_seed(4)
     x = torch.randn(M, K, device="cuda", generator=g).bfloat16()
     wg = (torch.randn(I, K, device="cuda", generator=g) / K ** 0.5).bfloat16()
     wu = (torch.randn(I, K, device="cuda", generator=g) / K ** 0.5).bfloat16()
     w = torch.stack([wg, wu], 1).reshape(2 * I, K).contiguous()
-    _lib.lib().vllm_gemm_set_variant(variant)
-    try:
+    with _lib.knob("gemm_set_variant", variant):
         out = ops().linear(x, w, act="swiglu")
-    finally:
-        _lib.lib().vllm_gemm_set_variant(0)
     ref = torch.nn.functional.silu(x.float() @ wg.float().T) * (x.float() @ wu.float().T)
     assert out.shape == (M, I)
     close(out, ref)
@@ -184,26 +176,23 @@ def test_rope_matches_hf_formula():
 
 
 # ---- backward GEMMs: MN-major operands (dgrad / wgrad without transposed copies) ----
-@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("variant", [pytest.param(v, id=t) for t, v in TILES.items()])
 @pytest.mark.parametrize("T,out_f,in_f", [(512, 256, 384), (2048, 4096, 4096), (300, 1376, 4096), (1000, 520, 200)])
 def test_gemm_tn_dgrad_wgrad_match_torch(T, out_f, in_f, variant):
     """dx = dy . W and dW = dy^T . x through vllm_gemm_bf16_tn vs fp32 torch on the same bf16 inputs (one bf16 output
     rounding + 1e-3 max|ref|), both tile widths, ragged M / N / K tails."""
-    from visionllm_b200 import _lib, ops
+    from visionllm_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(T + out_f)
     dy = (torch.randn(T, out_f, device="cuda", generator=g) * 0.5).bfloat16()
     x = (torch.randn(T, in_f, device="cuda", generator=g) * 0.5).bfloat16()
     w = (torch.randn(out_f, in_f, device="cuda", generator=g) * 0.05).bfloat16()
-    _lib.lib().vllm_gemm_set_variant(variant)
-    try:
+    with _lib.knob("gemm_set_variant", variant):
         dx = ops.gemm_tn(dy, w, b_mn=True)
         dw = ops.gemm_tn(dy, x, a_mn=True, b_mn=True, out_dtype=torch.float32)
         y = ops.gemm_tn(x, w)                                            # both K-major == ops.linear
         xt = torch.zeros((in_f, (T + 7) // 8 * 8), dtype=torch.bfloat16, device="cuda")   # [K, M] with a 16-byte row pitch
         xt[:, :T] = x.t()
         at = ops.gemm_tn(xt[:, :T], w, a_mn=True)                       # MN-major A alone
-    finally:
-        _lib.lib().vllm_gemm_set_variant(0)
     ref_dx = dy.float() @ w.float()
     ref_dw = dy.float().t() @ x.float()
     ref_y = x.float() @ w.float().t()

@@ -10,6 +10,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import msda_oracle as O  # noqa: E402
+from visionllm_b200 import _lib  # noqa: E402
 
 
 def _ext():
@@ -97,20 +98,16 @@ def test_strict_fp64_bit_exact_vs_oracle(case):
 
 
 # ---- fast kernel: indices bit-exact, values within fp32 reassociation noise ---------
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4])
+@pytest.mark.parametrize("variant", [_lib.MSDA_DEFAULT, _lib.MSDA_NO_HINT])
 @pytest.mark.parametrize("case", [c for c in CASES if c[3] == 32 and len(c[0]) * c[5] <= 32],
                          ids=lambda c: f"L{len(c[0])}P{c[5]}Lq{c[4]}")
 def test_fast_fp32_vs_oracle(case, variant):
     ext = _ext()
-    from visionllm_b200 import _lib
     value, shapes, lsi, loc, attw = make_case(*case, seed=5)
     ref = O.forward_kernel_semantics(value, shapes, lsi, loc, attw)
     v, sh, ls, lo, w = _dev(value, shapes, lsi, loc, attw)
-    _lib.lib().vllm_msda_set_variant(variant)
-    try:
+    with _lib.knob("msda_set_variant", variant):
         out = ext.ms_deform_attn_forward(v, sh, ls, lo, w, 64).cpu().numpy()
-    finally:
-        _lib.lib().vllm_msda_set_variant(0)
     # north-star tolerance is 1e-3 rel; reassociation of <= 4*K fp32 terms gives ~1e-6
     assert np.abs(out - ref).max() <= 1e-5 * max(1.0, np.abs(ref).max())
 
@@ -211,12 +208,8 @@ def test_full_size_fast_equals_strict_and_hint_invariance():
     strict = ext.ms_deform_attn_forward(value, shapes, lsi, loc, attw, 64, flags=1)
     assert (fast - strict).abs().max().item() <= 1e-5 * strict.abs().max().item()
     # the host shape hint only re-orders work: results must be bit-identical without it
-    from visionllm_b200 import _lib
-    _lib.lib().vllm_msda_set_variant(4)
-    try:
+    with _lib.knob("msda_set_variant", _lib.MSDA_NO_HINT):
         nohint = ext.ms_deform_attn_forward(value, shapes, lsi, loc, attw, 64)
-    finally:
-        _lib.lib().vllm_msda_set_variant(0)
     assert torch.equal(fast, nohint)
 
 
@@ -240,7 +233,7 @@ def test_full_size_linearity_in_value():
 
 
 # ---- "fast mode" (SURVEY 8d cfg 2b): bf16 value read in place ----
-@pytest.mark.parametrize("case", ["enc", "dec", "oob", "odd_points"])
+@pytest.mark.parametrize("case", ["enc", "dec", "oob", "odd_points", "points2", "generic_k"])
 @pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
 def test_bf16_value_matches_fp32_op_on_upcast_value(case, out_dtype):
     """ms_deform_attn_forward_bf16(value_bf16) == ms_deform_attn_forward(value_bf16.float()) (exact upcast inside the
@@ -249,7 +242,8 @@ def test_bf16_value_matches_fp32_op_on_upcast_value(case, out_dtype):
     from oracle import msda_oracle as O
     g = torch.Generator(device="cuda").manual_seed(7)
     shapes_l = [(20, 27), (10, 14), (5, 7), (3, 4)]
-    L, P = (4, 4) if case != "odd_points" else (4, 3)
+    L, P = {"odd_points": (4, 3), "points2": (4, 2), "generic_k": (3, 2)}.get(case, (4, 4))   # all but (4, 4): generic-K kernel
+    shapes_l = shapes_l[:L]
     shapes = torch.tensor(shapes_l, dtype=torch.int64, device="cuda")
     lsi = torch.cat((shapes.new_zeros(1), shapes.prod(1).cumsum(0)[:-1]))
     S = int(shapes.prod(1).sum())
@@ -270,84 +264,6 @@ def test_bf16_value_matches_fp32_op_on_upcast_value(case, out_dtype):
         assert (fast - orc).abs().max().item() <= 1e-5 * scale
     else:
         assert torch.equal(fast, ref.bfloat16()) or ((fast.float() - ref).abs() <= 2.0 ** -8 * ref.abs() + 1e-5 * scale).all()
-
-
-# ---- paired-row fast mode: two line fetches per sample ----
-@pytest.mark.parametrize("case", ["enc", "dec", "oob", "points2", "generic_k"])
-@pytest.mark.parametrize("out_dtype", [torch.float32, torch.bfloat16])
-def test_pairs_mode_matches_fp32_op_on_upcast_value(case, out_dtype):
-    """pack_pairs + forward_pairs == ms_deform_attn_forward(value_bf16.float()) up to fp32 summation order, incl. samples
-    hanging over every edge (w_low = -1 re-based pair, zero partner at the right edge, rows -1 / H predicated off)."""
-    import visionllm_b200.msda as ext
-    from oracle import msda_oracle as O
-    g = torch.Generator(device="cuda").manual_seed(11)
-    shapes_l = [(20, 27), (10, 14), (5, 7), (3, 4)]
-    L, P = {"points2": (4, 2), "generic_k": (3, 2)}.get(case, (4, 4))
-    shapes_l = shapes_l[:L]
-    shapes = torch.tensor(shapes_l, dtype=torch.int64, device="cuda")
-    lsi = torch.cat((shapes.new_zeros(1), shapes.prod(1).cumsum(0)[:-1]))
-    S = int(shapes.prod(1).sum())
-    N, M, D = 3, 8, 32
-    Lq = S if case != "dec" else 37
-    value = torch.randn(N, S, M, D, device="cuda", generator=g).bfloat16()
-    spread = 1.6 if case == "oob" else 1.05
-    loc = (torch.rand(N, Lq, M, L, P, 2, device="cuda", generator=g) - 0.5) * spread + 0.5
-    aw = torch.softmax(torch.randn(N, Lq, M, L * P, device="cuda", generator=g), -1).view(N, Lq, M, L, P).contiguous()
-    pairs = ext.ms_deform_attn_pack_pairs(value, shapes, lsi)
-    # layout contract of the pack kernel
-    assert not pairs[-1].any()                      # the all-zero line off-map corners read
-    pairs5 = pairs[:-1].view(N, S, M, 2, D)
-    assert torch.equal(pairs5[:, :, :, 0], value)
-    right = torch.zeros_like(value)
-    for (H, W), st in zip(shapes_l, lsi.tolist()):
-        v = value[:, st:st + H * W].view(N, H, W, M, D)
-        r = torch.zeros_like(v); r[:, :, :-1] = v[:, :, 1:]
-        right[:, st:st + H * W] = r.view(N, H * W, M, D)
-    assert torch.equal(pairs5[:, :, :, 1], right)
-    fast = ext.ms_deform_attn_forward_pairs(pairs, shapes, lsi, loc, aw, out_dtype)
-    ref = ext.ms_deform_attn_forward(value.float(), shapes, lsi, loc, aw, 64)
-    orc = torch.from_numpy(O.forward_kernel_semantics(value.float().cpu().numpy(), shapes.cpu().numpy(), lsi.cpu().numpy(),
-                                                      loc.cpu().numpy(), aw.cpu().numpy())).cuda()
-    assert fast.dtype == out_dtype and fast.shape == ref.shape
-    scale = orc.abs().max().item()
-    if out_dtype == torch.float32:
-        assert (fast - ref).abs().max().item() <= 1e-5 * scale
-        assert (fast - orc).abs().max().item() <= 1e-5 * scale
-    else:
-        assert ((fast.float() - ref).abs() <= 2.0 ** -8 * ref.abs() + 1e-5 * scale).all()
-
-
-def test_pairs_mode_skips_out_of_map_corners_like_the_reference():
-    """A corner outside the map is never read (reference .cuh:31-58): poison everything a sample at the map border must
-    not touch with NaN and compare with the fp32 operator on the same poisoned value."""
-    import visionllm_b200.msda as ext
-    shapes = torch.tensor([[6, 5], [3, 4]], dtype=torch.int64, device="cuda")
-    lsi = torch.tensor([0, 30], dtype=torch.int64, device="cuda")
-    S, N, M, D, L, P = 42, 1, 2, 32, 2, 2
-    g = torch.Generator(device="cuda").manual_seed(3)
-    value = torch.randn(N, S, M, D, device="cuda", generator=g).bfloat16()
-    value[:, 5] = float("nan")       # pixel (1, 0) of level 0: the row-wrapped "right neighbour" of pixel (0, 4)
-    value[:, 29] = float("nan")      # last pixel of level 0
-    # queries whose samples hang over the right / top / left borders of level 0, and far outside
-    pts = torch.tensor([[[0.99, 0.05], [0.95, 0.05]], [[-0.05, 0.3], [0.3, -0.05]], [[1.15, 0.5], [0.5, 1.3]]],
-                       device="cuda")                                        # [Lq = 3, P = 2, (x, y)]
-    loc = pts.view(1, 3, 1, 1, 2, 2).expand(N, 3, M, L, 2, 2).contiguous()
-    aw = torch.full((N, 3, M, L, P), 1.0 / (L * P), device="cuda")
-    pairs = ext.ms_deform_attn_pack_pairs(value, shapes, lsi)
-    fast = ext.ms_deform_attn_forward_pairs(pairs, shapes, lsi, loc, aw, torch.float32)
-    ref = ext.ms_deform_attn_forward(value.float(), shapes, lsi, loc, aw, 64)
-    assert torch.equal(torch.isnan(fast), torch.isnan(ref))
-    ok = ~torch.isnan(ref)
-    assert (fast[ok] - ref[ok]).abs().max().item() <= 1e-5
-
-
-def test_pairs_mode_full_size_constant_field():
-    import visionllm_b200.msda as ext
-    value, shapes, lsi, loc, attw = _full_size(N=2)
-    loc = loc.clamp(0.2, 0.8).contiguous()
-    pairs = ext.ms_deform_attn_pack_pairs(torch.ones_like(value).bfloat16(), shapes, lsi)
-    out = ext.ms_deform_attn_forward_pairs(pairs, shapes, lsi, loc, attw, torch.float32)
-    assert (out - 1.0).abs().max().item() < 1e-5
 
 
 def test_bf16_value_rejects_unsupported():

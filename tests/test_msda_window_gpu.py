@@ -1,6 +1,6 @@
 """GPU: the TMA-staged window kernel of the encoder shape (csrc/msda_win.cu) against the C oracle and against the
 global-memory warp-gather kernel it replaces.  The window only decides WHERE a corner row is read from (shared-memory
-window filled by TMA vs global memory), never what is computed, so the two paths must agree BIT FOR BIT for any
+window filled by TMA or by cp.async vs global memory), never what is computed, so the two paths must agree BIT FOR BIT for any
 window size -- including windows so small that most (query, head) pairs take the in-kernel fallback."""
 import numpy as np
 import pytest
@@ -9,6 +9,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import msda_oracle as O  # noqa: E402
+from visionllm_b200 import _lib  # noqa: E402
 
 
 def enc_case(shapes_l, N, M, sigma, seed, outlier_frac=0.02, P=4, valid_ratio=None):
@@ -36,24 +37,17 @@ def enc_case(shapes_l, N, M, sigma, seed, outlier_frac=0.02, P=4, valid_ratio=No
     return value, shapes, lsi, loc, attw
 
 
-def run(value, shapes, lsi, loc, attw, variant=0, window=(0, 0, 0), out_dtype=None, tma_fill=False):
-    """value fp32 -> ms_deform_attn_forward; value bf16 -> ms_deform_attn_forward_bf16(out_dtype)."""
+def run(value, shapes, lsi, loc, attw, variant=_lib.MSDA_DEFAULT, window=(0, 0, 0), out_dtype=None, fill=-1):
+    """value fp32 -> ms_deform_attn_forward; value bf16 -> ms_deform_attn_forward_bf16(out_dtype).  fill: the level mask of
+    vllm_msda_set_window_fill; -1 leaves the library's default (every level by TMA), 0 = every level by cooperative cp.async."""
     import visionllm_b200.msda as ext
-    from visionllm_b200 import _lib
-    L_ = _lib.lib()
-    if value.dtype == torch.float32 and variant == 0:
-        variant = 33                                   # fp32 rows: the window kernel is opt-in (the default is the patch kernel)
-    L_.vllm_msda_set_variant(variant)
-    L_.vllm_msda_set_window(*window)
-    L_.vllm_msda_set_window_fill(1 if tma_fill else 0)
-    try:
+    if value.dtype == torch.float32 and variant == _lib.MSDA_DEFAULT:
+        variant = _lib.MSDA_FP32_WINDOW                # fp32 rows: the window kernel is opt-in (the default is the patch kernel)
+    with _lib.knob("msda_set_variant", variant), _lib.knob("msda_set_window", *window), \
+            _lib.knob("msda_set_window_fill", fill):
         if value.dtype == torch.float32:
             return ext.ms_deform_attn_forward(value, shapes, lsi, loc, attw, 64)
         return ext.ms_deform_attn_forward_bf16(value, shapes, lsi, loc, attw, out_dtype)
-    finally:
-        L_.vllm_msda_set_variant(0)
-        L_.vllm_msda_set_window(0, 0, 0)
-        L_.vllm_msda_set_window_fill(-1)
 
 
 def oracle(value, shapes, lsi, loc, attw):
@@ -78,10 +72,11 @@ def test_window_kernel_vs_oracle_and_bit_identical_to_global_path(pyr, mode):
         value = value.bfloat16()
     od = {"f32": None, "bf16_f32out": torch.float32, "bf16_bf16out": torch.bfloat16}[mode]
     win = run(value, shapes, lsi, loc, attw, out_dtype=od)
-    glob = run(value, shapes, lsi, loc, attw, variant=32 if mode != "f32" else 4, out_dtype=od)
+    glob = run(value, shapes, lsi, loc, attw, variant=_lib.MSDA_BF16_NO_WINDOW if mode != "f32" else _lib.MSDA_NO_HINT,
+               out_dtype=od)
     assert torch.equal(win, glob), (win.float() - glob.float()).abs().max().item()
-    # the two window-fill mechanisms (cooperative cp.async, default; one TMA box per level) give the same bits
-    assert torch.equal(run(value, shapes, lsi, loc, attw, out_dtype=od, tma_fill=True), win)
+    # the two window-fill mechanisms (one TMA box per level, the default; cooperative cp.async) give the same bits
+    assert torch.equal(run(value, shapes, lsi, loc, attw, out_dtype=od, fill=0), win)
     ref = oracle(value, shapes, lsi, loc, attw)
     scale = ref.abs().max().item()
     if win.dtype == torch.float32:
@@ -94,8 +89,8 @@ def test_window_kernel_vs_oracle_and_bit_identical_to_global_path(pyr, mode):
 def test_result_does_not_depend_on_the_window_geometry(window):
     """Tiny windows push most pairs through the in-kernel global fallback, large ones none: same bits every time."""
     value, shapes, lsi, loc, attw = enc_case(PYRAMIDS["npot"], N=1, M=8, sigma=0.04, seed=3, outlier_frac=0.05)
-    base32 = run(value, shapes, lsi, loc, attw, variant=4)
-    base16 = run(value.bfloat16(), shapes, lsi, loc, attw, variant=32, out_dtype=torch.float32)
+    base32 = run(value, shapes, lsi, loc, attw, variant=_lib.MSDA_NO_HINT)
+    base16 = run(value.bfloat16(), shapes, lsi, loc, attw, variant=_lib.MSDA_BF16_NO_WINDOW, out_dtype=torch.float32)
     assert torch.equal(run(value, shapes, lsi, loc, attw, window=window), base32)
     assert torch.equal(run(value.bfloat16(), shapes, lsi, loc, attw, window=window, out_dtype=torch.float32), base16)
 
@@ -110,7 +105,7 @@ def test_padded_image_valid_ratios_and_pixel_centre_references():
         win = run(value, shapes, lsi, loc, attw)
         ref = oracle(value, shapes, lsi, loc, attw)
         assert (win - ref).abs().max().item() <= 1e-5 * max(1.0, ref.abs().max().item())
-        assert torch.equal(win, run(value, shapes, lsi, loc, attw, variant=4))
+        assert torch.equal(win, run(value, shapes, lsi, loc, attw, variant=_lib.MSDA_NO_HINT))
 
 
 def test_out_of_range_samples_and_unsampled_nans_do_not_leak():
@@ -148,13 +143,13 @@ def test_full_size_encoder_shape_properties():
     hs = shapes.cpu()
     import visionllm_b200.msda as ext
     win = run(value, shapes, lsi, loc, attw)
-    assert torch.equal(win, run(value, shapes, lsi, loc, attw, variant=4))
+    assert torch.equal(win, run(value, shapes, lsi, loc, attw, variant=_lib.MSDA_NO_HINT))
     assert torch.equal(win, ext.ms_deform_attn_forward(value, shapes, lsi, loc, attw, 64, host_shapes=hs))   # default path
     strict = ext.ms_deform_attn_forward(value, shapes, lsi, loc, attw, 64, flags=ext.STRICT)
     assert (win - strict).abs().max().item() <= 1e-5 * strict.abs().max().item()
     v16 = value.bfloat16()
     w16 = ext.ms_deform_attn_forward_bf16(v16, shapes, lsi, loc, attw, torch.float32)
-    assert torch.equal(w16, run(v16, shapes, lsi, loc, attw, variant=32, out_dtype=torch.float32))
+    assert torch.equal(w16, run(v16, shapes, lsi, loc, attw, variant=_lib.MSDA_BF16_NO_WINDOW, out_dtype=torch.float32))
     assert (w16 - ext.ms_deform_attn_forward(v16.float(), shapes, lsi, loc, attw, 64, flags=ext.STRICT)).abs().max().item() \
         <= 1e-5 * strict.abs().max().item()
     ones = torch.ones_like(value)

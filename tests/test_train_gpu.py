@@ -8,28 +8,26 @@ import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
+from visionllm_b200 import _lib  # noqa: E402
+
 
 def rel(a, b):
     return float(torch.linalg.norm(a.float() - b.float()) / (torch.linalg.norm(b.float()) + 1e-30))
 
 
-@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("variant", [pytest.param(_lib.GEMM_DEFAULT, id="1"), pytest.param(_lib.GEMM_WIDE_TILE, id="2")])   # id: tile width / 128 columns
 def test_batched_gemm_forms_of_the_attention_backward(variant):
-    from visionllm_b200 import _lib
     from visionllm_b200.train import gemm_batched
     g = torch.Generator(device="cuda").manual_seed(0)
     BH, T, D = 3, 512, 128
     q, k = ((torch.randn(BH, T, D, device="cuda", generator=g) * 0.3).bfloat16() for _ in range(2))
     p = (torch.randn(BH, T, T, device="cuda", generator=g) * 0.3).bfloat16().tril()       # causal: zero above the diagonal
-    _lib.lib().vllm_gemm_set_variant(variant)
-    try:
+    with _lib.knob("gemm_set_variant", variant):
         s = gemm_batched(q.view(BH * T, D), k.view(BH * T, D), BH, T, T, D, causal=1).view(BH, T, T)
         s_full = gemm_batched(q.view(BH * T, D), k.view(BH * T, D), BH, T, T, D).view(BH, T, T)
         dv = gemm_batched(p.view(BH * T, T), q.view(BH * T, D), BH, T, D, T, a_mn=True, b_mn=True, causal=2).view(BH, T, D)
         dv_nc = gemm_batched(p.view(BH * T, T), q.view(BH * T, D), BH, T, D, T, a_mn=True, b_mn=True).view(BH, T, D)
         dq = gemm_batched(p.view(BH * T, T), k.view(BH * T, D), BH, T, D, T, b_mn=True, causal=3).view(BH, T, D)
-    finally:
-        _lib.lib().vllm_gemm_set_variant(0)
     ref_s = q.float() @ k.float().transpose(1, 2)
     tol = lambda ref: 2.0 ** -8 * ref.abs() + 1e-3 * ref.abs().max()  # noqa: E731
     assert ((s_full.float() - ref_s).abs() <= tol(ref_s)).all()

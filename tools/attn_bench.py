@@ -29,14 +29,13 @@ for name, (B, T, H, causal) in SHAPES.items():
     fl = 4.0 * B * H * T * T * 128 * (0.5 if causal else 1.0)
     r = {}
     for var, nm in ((0, "wgmma"), (1, "warp_mma")):
-        _lib.lib().vllm_attention_set_variant(var)
         try:
-            ms = timeit(lambda: ops.attention(q, k, v, causal=causal))
+            with _lib.knob("attention_set_variant", var):
+                ms = timeit(lambda: ops.attention(q, k, v, causal=causal))
             r[nm + "_tflops"] = fl / ms / 1e9
             r[nm + "_ms"] = ms
         except Exception as e:
             r[nm + "_error"] = str(e)
-    _lib.lib().vllm_attention_set_variant(0)
     qt, kt, vt = (t.transpose(1, 2) for t in (q, k, v))
     ms = timeit(lambda: torch.nn.functional.scaled_dot_product_attention(qt, kt, vt, is_causal=causal))
     r["torch_sdpa_tflops"] = fl / ms / 1e9

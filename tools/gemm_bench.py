@@ -30,14 +30,13 @@ for name, (M, N, K) in SHAPES.items():
     out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
     fl = 2.0 * M * N * K
     r = {}
-    for v, nm in ((1, "tile128x128"), (2, "tile128x256")):
-        _lib.lib().vllm_gemm_set_variant(v)
+    for v, nm in ((_lib.GEMM_DEFAULT, "tile128x128"), (_lib.GEMM_WIDE_TILE, "tile128x256")):
         try:
-            ms = timeit(lambda: ops.linear(x, w, out=out))
+            with _lib.knob("gemm_set_variant", v):
+                ms = timeit(lambda: ops.linear(x, w, out=out))
             r[f"{nm}_tflops"] = fl / ms / 1e9
         except Exception as e:
             r[f"{nm}_error"] = str(e)
-    _lib.lib().vllm_gemm_set_variant(0)
     ms = timeit(lambda: torch.matmul(x, w.T, out=out))
     r["cublas_tflops"] = fl / ms / 1e9
     res[name] = r

@@ -5,6 +5,7 @@ the ONLY compute path of this package: a missing library is an ImportError at
 first use, never a silent fallback (the reference silently falls back to
 grid_sample, grounding_dino/modeling_ov_grounding_dino_mask_dn.py:777-779).
 """
+import contextlib
 import ctypes
 import os
 import threading
@@ -26,8 +27,6 @@ _SIGNATURES = {
     "vllm_version": (ctypes.c_char_p, []),
     "vllm_msda_forward_f32": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp, ci, vp]),
     "vllm_msda_forward_bf16v": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp]),
-    "vllm_msda_pack_pairs_bf16": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]),
-    "vllm_msda_forward_pairs": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp]),
     "vllm_msda_forward_f64": (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_msda_backward_f32": (ci, [vp] * 9 + [ci] * 7 + [vp]),
     "vllm_msda_backward_f64": (ci, [vp] * 9 + [ci] * 7 + [vp]),
@@ -62,7 +61,6 @@ _SIGNATURES = {
     "vllm_attn_ds_bf16": (ci, [vp, vp, cll, cll, ci, cf, vp]),
     "vllm_ce_loss_f32": (ci, [vp, cll, vp, vp, cll, ci, vp, vp, cll, vp]),
     "vllm_gemm_set_variant": (ci, [ci]),
-    "vllm_gemm_set_group_m": (ci, [ci]),
     "vllm_rmsnorm_bf16": (ci, [vp, cll, vp, vp, cll, cll, ci, cf, vp]),
     "vllm_layernorm_bf16": (ci, [vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),
     "vllm_layernorm_gelu_bf16": (ci, [vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),
@@ -73,8 +71,6 @@ _SIGNATURES = {
     "vllm_dwconv_nhwc_bf16": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]),
     "vllm_rope_bf16": (ci, [vp, cll, vp, vp, cll, ci, ci, vp]),
     "vllm_groupnorm_workspace_bytes": (cll, [ci, ci]),
-    "vllm_groupnorm_nhwc_bf16": (ci, [vp, vp, vp, vp, ci, cll, ci, ci, cf, ci, vp, cll, vp]),
-    "vllm_upsample_add_nhwc_bf16": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_upsample_add_nhwc_bf16_ex": (ci, [vp, cll, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_groupnorm_nhwc_bf16_grid": (ci, [vp, vp, vp, vp, ci, cll, cll, cll, cll, ci, ci, cf, ci, vp, cll, vp]),
     "vllm_attention_bf16": (ci, [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cll, cll, cll, cll, cll, cll, cll, cll,
@@ -95,6 +91,15 @@ _SIGNATURES = {
     "vllm_tp_wait": (ci, [vp, ctypes.c_uint, vp]),
     "vllm_tp_signal": (ci, [vp, ci, ctypes.c_uint, vp]),
 }
+
+
+# values of vllm_msda_set_variant / vllm_gemm_set_variant (include/vllm_b200.h)
+MSDA_DEFAULT, MSDA_NO_HINT, MSDA_BF16_NO_WINDOW, MSDA_FP32_WINDOW = 0, 4, 32, 33
+GEMM_DEFAULT, GEMM_WIDE_TILE = 0, 2
+
+# the process-global path / tuning setters and the arguments that restore the library's own choice
+_KNOB_DEFAULTS = {"msda_set_variant": (MSDA_DEFAULT,), "msda_set_window": (0, 0, 0), "msda_set_window_fill": (-1,),
+                  "gemm_set_variant": (GEMM_DEFAULT,), "attention_set_variant": (0,)}
 
 
 class VllmB200Error(RuntimeError):
@@ -136,6 +141,21 @@ def check(rc, what):
     if rc < 0:
         raise VllmB200Error(f"{what}: {_ERR.get(rc, 'error')} (rc={rc})")
     raise VllmB200Error(f"{what}: CUDA error {rc} at launch")
+
+
+@contextlib.contextmanager
+def knob(name, *values):
+    """`with knob("msda_set_variant", MSDA_NO_HINT): ...` calls vllm_<name>(*values), raises if the library rejects them,
+    and puts the default back on exit -- the knobs are process-global, so a value left behind would leak into every
+    later call."""
+    fn = getattr(lib(), "vllm_" + name)
+    rc = fn(*values)
+    if rc != 0:
+        raise VllmB200Error(f"vllm_{name}{values}: {_ERR.get(rc, 'error')} (rc={rc})")
+    try:
+        yield
+    finally:
+        fn(*_KNOB_DEFAULTS[name])
 
 
 def launch_count():

@@ -24,6 +24,7 @@
 // Tiles are visited in groups of GROUP_M row-blocks so concurrently running CTAs share B (weights) in L2.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "vllm_b200.h"   // VLLM_GEMM_* variant names
 
 namespace {
 
@@ -41,7 +42,7 @@ struct GemmArgs {
   int act; int out_f32;
   const unsigned char* row_keep;   // optional [M]: rows with 0 are written as exact zeros (value.masked_fill of the MSDA module)
   int tiles_m, tiles_n;
-  int group_m;           // row-blocks per rasterisation group (see pick_group_m)
+  int group_m;           // row-blocks per rasterisation group (see launch_gemm)
   // Implicit convolution over a zero-padded channels-last image (vllm_conv_rows_bf16): the K axis is a_segs segments
   // of a_seg_kb k-blocks; segment s reads A rows shifted by s * a_seg_rows (one image row of the padded map), and a
   // row of the A tensor map spans kw consecutive pixels (row pitch = C elements, row length = kw*C: rows overlap).
@@ -333,20 +334,16 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   }
 }
 
-// Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so one wave of
-// CTAs covers a near-square patch of tiles (minimal A+B bytes per wave).  The knob remains for sweeps.
-int g_group_m_override = 0;
 // SM budgets (0 = every SM): a persistent GEMM CTA owns its SM (384 threads with the whole register file between them), so a
 // link-bound kernel of another stream -- the peer pushes of the tensor-parallel exchange -- can only overlap a GEMM on SMs
 // the GEMM's grid leaves free.  g_sm_limit caps every launch, g_scatter_sm_limit the scatter GEMM (vllm_gemm_bf16_scatter),
 // whose epilogue stores ride NVLink while the other micro-batch's GEMM runs beside it (visionllm_b200/tp.py).
 int g_sm_limit = 0, g_scatter_sm_limit = 0;
-int pick_group_m(int, int, long long) { return g_group_m_override > 0 ? g_group_m_override : 8; }
 
-// 0: auto = 128 x 128 tiles (faster than 128 x 256 at every hot-path shape measured on an H100, README.md);
-// 1 / 2: force the 128- / 256-column tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its receivers
-// count arrivals per such tile.
-int g_gemm_variant = 0;
+// VLLM_GEMM_DEFAULT: 128 x 128 tiles (faster than 128 x 256 at every hot-path shape measured on an H100, README.md);
+// VLLM_GEMM_WIDE_TILE forces the 256-column tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its
+// receivers count arrivals per such tile.
+int g_gemm_variant = VLLM_GEMM_DEFAULT;
 
 template <int BN>
 int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cudaStream_t st, long long a_rows = -1,
@@ -369,7 +366,9 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
   const int limit = g.sc_rows ? (g_scatter_sm_limit > 0 ? g_scatter_sm_limit : g_sm_limit) : g_sm_limit;
   if (limit > 0 && limit < sms) sms = limit;
   const int ctas = sms < n_tiles ? sms : n_tiles;
-  g.group_m = pick_group_m(sms, g.tiles_n, (long long)g.N * g.K * 2);
+  // Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so one wave of
+  // CTAs covers a near-square patch of tiles (minimal A+B bytes per wave).
+  g.group_m = 8;
   static bool attr_set[64] = {false};
   bool* set = vllm_device_flag(attr_set);
   if (!set || !*set) {
@@ -385,7 +384,7 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
 int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmArgs& g, cudaStream_t st, long long a_rows = -1,
                      int a_cols = -1) {
   // the receivers of a scatter GEMM count 8 arrivals per 128 x 256 tile (visionllm_b200/tp.py)
-  const bool wide = g.sc_rows || g_gemm_variant == 2;
+  const bool wide = g.sc_rows || g_gemm_variant == VLLM_GEMM_WIDE_TILE;
   return wide ? launch_gemm<256>(A, lda, B, ldb, g, st, a_rows, a_cols) : launch_gemm<128>(A, lda, B, ldb, g, st, a_rows, a_cols);
 }
 
@@ -393,8 +392,11 @@ int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmA
 
 extern "C" {
 
-int vllm_gemm_set_variant(int v) { g_gemm_variant = (v == 1 || v == 2) ? v : 0; return VLLM_OK; }
-int vllm_gemm_set_group_m(int gm) { g_group_m_override = gm; return VLLM_OK; }
+int vllm_gemm_set_variant(int v) {
+  if (v != VLLM_GEMM_DEFAULT && v != VLLM_GEMM_WIDE_TILE) return VLLM_EINVAL;
+  g_gemm_variant = v;
+  return VLLM_OK;
+}
 int vllm_gemm_set_sm_limit(int all_gemms, int scatter_gemm) {
   if (all_gemms < 0 || scatter_gemm < 0) return VLLM_EINVAL;
   g_sm_limit = all_gemms; g_scatter_sm_limit = scatter_gemm;

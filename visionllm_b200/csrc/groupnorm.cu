@@ -232,14 +232,6 @@ int vllm_groupnorm_nhwc_bf16_grid(const void* x, void* y, const void* gamma, con
   return VLLM_OK;
 }
 
-int vllm_groupnorm_nhwc_bf16(const void* x, void* y, const void* gamma, const void* beta, int batch, long long hw,
-                             int channels, int groups, float eps, int relu, void* workspace, long long workspace_bytes,
-                             void* stream) {
-  if (hw < 0) return VLLM_EINVAL;
-  return vllm_groupnorm_nhwc_bf16_grid(x, y, gamma, beta, batch, hw ? 1 : 0, hw, hw, hw, channels, groups, eps, relu, workspace,
-                                       workspace_bytes, stream);
-}
-
 int vllm_upsample_add_nhwc_bf16_ex(const void* top, long long top_image_pitch, const void* lateral, void* out, int batch, int in_h,
                                    int in_w, int out_h, int out_w, int channels, int out_pad, void* stream) {
   if (batch < 0 || in_h <= 0 || in_w <= 0 || out_h <= 0 || out_w <= 0 || channels <= 0 || out_pad < 0) return VLLM_EINVAL;
@@ -257,12 +249,6 @@ int vllm_upsample_add_nhwc_bf16_ex(const void* top, long long top_image_pitch, c
       (float)in_h / (float)out_h, (float)in_w / (float)out_w, top_image_pitch, out_pad);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
-}
-
-int vllm_upsample_add_nhwc_bf16(const void* top, const void* lateral, void* out, int batch, int in_h, int in_w, int out_h,
-                                int out_w, int channels, void* stream) {
-  return vllm_upsample_add_nhwc_bf16_ex(top, (long long)in_h * in_w * channels, lateral, out, batch, in_h, in_w, out_h, out_w,
-                                        channels, 0, stream);
 }
 
 }  // extern "C"

@@ -36,6 +36,7 @@
 // into an FMA.  msda_geom() uses __fmul_rn/__fsub_rn and is shared by both
 // kernels and by the index-dump entry point the parity tests use.
 #include "msda_common.cuh"
+#include "vllm_b200.h"   // VLLM_MSDA_* variant names
 
 // ---------------------------------------------------------------------------
 // Strict kernel: reference mapping, reference order, no contraction.
@@ -313,196 +314,6 @@ msda_fwd_warp_kernel(const ValT* __restrict__ value, const int64_t* __restrict__
 
 
 // ---------------------------------------------------------------------------
-// Paired-row fast mode (bf16 value).  The gather is bound by L1 wavefronts (one 128-byte line per warp-instruction
-// slot), not by bytes: the four corners of a sample are four different lines in the reference layout, in fp32 (128 B
-// rows) and in bf16 (64 B rows, half of every line wasted) alike.  msda_pack_pairs_kernel rewrites the bf16 value
-// once per call into pairs[n][s][m][2][32]: slot 0 = value(s, m), slot 1 = value(s + 1, m) when pixel s + 1 lies in
-// the same image row (else 0), i.e. both horizontal corners of a sample in ONE aligned 128-byte line.  A sample then
-// costs two line fetches (rows h_low, h_low + 1) instead of four, and a warp instruction (32 x 16 B) covers two
-// samples.  Lane = (sample parity, row, column, channel octet); per-corner weights are the same products as in
-// msda_fwd_warp_kernel ((row weight * column weight) * attention weight), fp32 accumulation; corners outside the map
-// read an all-zero line appended behind the last pixel with weight 0 (w_low == -1 re-bases the pair on pixel 0), so a
-// NaN/Inf in a pixel the reference would not touch never reaches the sum.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-msda_pack_pairs_kernel(const __nv_bfloat16* __restrict__ value, __nv_bfloat16* __restrict__ pairs, long long n_chunks,
-                       const int64_t* __restrict__ shapes, const int64_t* __restrict__ lsi, int S, int M, int L) {
-  __shared__ int s_w[MSDA_MAX_LEVELS], s_start[MSDA_MAX_LEVELS];
-  if (threadIdx.x < L) {
-    s_w[threadIdx.x] = (int)shapes[2 * threadIdx.x + 1];
-    s_start[threadIdx.x] = (int)lsi[threadIdx.x];
-  }
-  __syncthreads();
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  if (blockIdx.x == 0 && threadIdx.x < 8)        // the all-zero line behind the last pixel: target of every off-map corner
-    *reinterpret_cast<uint4*>(pairs + n_chunks * 8 + threadIdx.x * 8) = make_uint4(0u, 0u, 0u, 0u);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_chunks; i += stride) {
-    const int oct = (int)(i & 3), slot = (int)((i >> 2) & 1);
-    const long long pm = i >> 3;               // (n*S + s)*M + m
-    const int m = (int)(pm % M);
-    const long long ns = pm / M;
-    const int sidx = (int)(ns % S);
-    int l = 0;
-    while (l + 1 < L && sidx >= s_start[l + 1]) ++l;
-    const int w = (sidx - s_start[l]) % s_w[l];
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (slot == 0 || w + 1 < s_w[l])
-      v = __ldg(reinterpret_cast<const uint4*>(value + ((ns + slot) * M + m) * 32 + oct * 8));
-    *reinterpret_cast<uint4*>(pairs + i * 8) = v;
-  }
-}
-
-constexpr int MSDA_PAIR_ROW = 32 + 2;   // int2 entries per (warp, row, column) slab: 32 samples + pad (slabs on different banks)
-
-template <int TH, int TW, int NW, int KC, int PC, typename OutT>
-__global__ void __launch_bounds__(NW * 32)
-msda_fwd_pair_kernel(const __nv_bfloat16* __restrict__ pairs, const int64_t* __restrict__ shapes,
-                     const int64_t* __restrict__ lsi, const float* __restrict__ loc,
-                     const float* __restrict__ attw, OutT* __restrict__ out,
-                     int S, int M, int L, int Lq, int P_rt, const __grid_constant__ MsdaTiling tl) {
-  constexpr int D = 32;
-  constexpr int TQ = TH * TW;
-  constexpr int QPW = TQ / NW;
-  static_assert(TQ % NW == 0, "tile must split evenly over warps");
-  __shared__ int s_h[MSDA_MAX_LEVELS], s_w[MSDA_MAX_LEVELS], s_start[MSDA_MAX_LEVELS];
-  __shared__ __align__(16) int2 s_meta[NW][4][MSDA_PAIR_ROW];   // [row*2 + column]: {byte offset, weight bits}; off-map corner -> zero line
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x < L) {
-    s_h[threadIdx.x] = (int)shapes[2 * threadIdx.x];
-    s_w[threadIdx.x] = (int)shapes[2 * threadIdx.x + 1];
-    s_start[threadIdx.x] = (int)lsi[threadIdx.x];
-  }
-  __syncthreads();
-
-  const int m = blockIdx.x % M;
-  const int tile = blockIdx.x / M;
-  const int b = blockIdx.y;
-  const int P = KC > 0 ? PC : P_rt;
-  const int K = KC > 0 ? KC : L * P_rt;           // even (host-checked)
-  const int G = (32 / K) < QPW ? (32 / K) : QPW;
-  const int pix_bytes = M * 128;                  // one pixel of the pair tensor: M heads x (2 x 32 bf16)
-
-  int lvl = 0, ty = 0, tx = 0;
-  if (tl.mode == 1) {
-    while (lvl + 1 < L && tile >= tl.tile_start[lvl + 1]) ++lvl;
-    const int lt = tile - tl.tile_start[lvl];
-    ty = lt / tl.tiles_w[lvl]; tx = lt % tl.tiles_w[lvl];
-  }
-  auto query_of = [&](int t) -> int {
-    if (tl.mode == 0) { const int q = tile * TQ + t; return q < Lq ? q : -1; }
-    const int py = ty * TH + t / TW, px = tx * TW + t % TW;
-    if (py >= tl.H[lvl] || px >= tl.W[lvl]) return -1;
-    return tl.q_start[lvl] + py * tl.W[lvl] + px;
-  };
-
-  // phase-2 role: lane = (sample parity, row, column, channel octet)
-  const int sp = lane >> 4, r = (lane >> 3) & 1, col = (lane >> 2) & 1, oct = lane & 3;
-  const char* vbl = reinterpret_cast<const char*>(pairs) + ((size_t)b * S * M + m) * 128 + (lane & 7) * 16;
-  const int g1 = lane / K, s1 = lane - g1 * K;    // phase-1 role
-  const int l1 = s1 / P;
-  // byte offset (relative to this CTA's (batch, head) base) of the all-zero line behind the last pixel of the tensor
-  const int zero_off = (int)(((long long)gridDim.y * S * M - ((long long)b * S * M + m)) * 128);
-
-  for (int t0 = 0; t0 < QPW; t0 += G) {
-    // ---- phase 1: one lane per sample -> two row entries ------------------
-    int q = -1;
-    if (g1 < G && t0 + g1 < QPW) q = query_of(warp * QPW + t0 + g1);
-    {
-      int2 e[4];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) e[c] = make_int2(zero_off, 0);   // weight 0 x zeros: contributes exactly 0
-      if (q >= 0) {
-        const size_t si = (((size_t)b * Lq + q) * M + m) * K + s1;
-        const float2 xy = ld_stream_f2(loc + 2 * si);
-        const float aw = ld_stream_f1(attw + si);
-        const int H = s_h[l1], W = s_w[l1];
-        const MsdaGeom<float> ge = msda_geom<float>(xy.x, xy.y, H, W);
-        if (ge.mask & 1) {
-          const float hh = 1.f - ge.lh, hw = 1.f - ge.lw;
-          // column slots: pixel w_low (slot 0) and w_low + 1 (slot 1); w_low == -1 re-bases the pair on pixel 0,
-          // whose slot 0 then carries the (h, w_high) corner
-          const bool left_out = ge.w_low < 0;
-          const int px = left_out ? 0 : ge.w_low;
-          const bool col1 = !left_out && ge.w_low + 1 <= W - 1;
-          const int off0 = (s_start[l1] + ge.h_low * W + px) * pix_bytes;
-          const int off1 = off0 + W * pix_bytes;
-          if (ge.h_low >= 0) {
-            e[0] = make_int2(off0, __float_as_int((left_out ? hh * ge.lw : hh * hw) * aw));
-            if (col1) e[1] = make_int2(off0, __float_as_int((hh * ge.lw) * aw));
-          }
-          if (ge.h_low + 1 <= H - 1) {
-            e[2] = make_int2(off1, __float_as_int((left_out ? ge.lh * ge.lw : ge.lh * hw) * aw));
-            if (col1) e[3] = make_int2(off1, __float_as_int((ge.lh * ge.lw) * aw));
-          }
-        }
-      }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) s_meta[warp][c][lane] = e[c];
-    }
-    __syncwarp();
-    // ---- phase 2: 2 samples x 2 rows x 128 B per warp instruction ----------
-    for (int g = 0; g < G && t0 + g < QPW; ++g) {
-      const int qg = __shfl_sync(0xffffffffu, q, g * K);
-      if (qg < 0) continue;  // warp-uniform
-      const int2* mp = &s_meta[warp][r * 2 + col][g * K + sp];
-      float acc[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-      auto fma8 = [&](const uint4& raw, float w) {
-        const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&raw);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float2 f = __bfloat1622float2(h[i]);
-          acc[2 * i] = fmaf(w, f.x, acc[2 * i]);
-          acc[2 * i + 1] = fmaf(w, f.y, acc[2 * i + 1]);
-        }
-      };
-      if constexpr (KC > 0 && (KC / 2) % 4 == 0) {
-        // batches of 4 line fetches in flight per lane, branch-free (predicated loads; an off corner contributes 0)
-#pragma unroll
-        for (int s0 = 0; s0 < KC / 2; s0 += 4) {
-          int2 me[4]; uint4 raw[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) me[j] = mp[2 * (s0 + j)];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) raw[j] = __ldg(reinterpret_cast<const uint4*>(vbl + (unsigned)me[j].x));
-#pragma unroll
-          for (int j = 0; j < 4; ++j) fma8(raw[j], __int_as_float(me[j].y));
-        }
-      } else {
-        for (int s = 0; s < K / 2; ++s) {
-          const int2 me = mp[2 * s];
-          fma8(__ldg(reinterpret_cast<const uint4*>(vbl + (unsigned)me.x)), __int_as_float(me.y));
-        }
-      }
-      // reduce-scatter over the 8 lanes that hold the same channel octet: 4 + 2 + 1 shuffles
-      float k4[4], k2[2];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float send = sp ? acc[j] : acc[j + 4];
-        const float recv = __shfl_xor_sync(0xffffffffu, send, 16);
-        k4[j] = (sp ? acc[j + 4] : acc[j]) + recv;
-      }
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const float send = r ? k4[j] : k4[j + 2];
-        const float recv = __shfl_xor_sync(0xffffffffu, send, 8);
-        k2[j] = (r ? k4[j + 2] : k4[j]) + recv;
-      }
-      const float send = col ? k2[0] : k2[1];
-      const float recv = __shfl_xor_sync(0xffffffffu, send, 4);
-      const float res = (col ? k2[1] : k2[0]) + recv;
-      const int ch = oct * 8 + sp * 4 + r * 2 + col;
-      OutT* op = out + (((size_t)b * Lq + qg) * M + m) * D + ch;
-      if constexpr (sizeof(OutT) == 4) *op = res;
-      else *op = __float2bfloat16(res);
-    }
-    __syncwarp();
-  }
-}
-
-// ---------------------------------------------------------------------------
 // Backward (SURVEY 8f rank 1): grad_value (atomics), grad_sampling_loc, grad_attn_weight.
 // Restates ms_deform_attn_col2im_bilinear + the col2im kernels (reference .cuh:66-124, 256-801): per output
 // channel c of a (b, q, m) pair and per sample: top_grad_value = grad_out * weight; each in-bounds corner
@@ -598,7 +409,7 @@ template <typename ValT, typename OutT>
 int msda_launch_window(const ValT* value, const int64_t* lsi, const float* loc, const float* attw, OutT* out, int N, int S,
                        int M, int L, int Lq, int P, const int64_t* host_shapes, cudaStream_t st);
 
-static int g_msda_variant = 0;  // bench/tuning knob, see vllm_msda_set_variant
+static int g_msda_variant = VLLM_MSDA_DEFAULT;  // see vllm_msda_set_variant
 
 static bool build_tiling(MsdaTiling& tl, const int64_t* host_shapes, int L, int Lq, int S, int TH, int TW) {
   tl.mode = 0;
@@ -638,25 +449,6 @@ static int launch_warp(const ValT* value, const int64_t* shapes, const int64_t* 
   return VLLM_OK;
 }
 
-
-template <int TH, int TW, int NW, typename OutT>
-static int launch_pair(const __nv_bfloat16* pairs, const int64_t* shapes, const int64_t* lsi, const float* loc,
-                       const float* attw, OutT* out, int N, int S, int M, int L, int Lq, int P,
-                       const int64_t* host_shapes, cudaStream_t st) {
-  MsdaTiling tl; memset(&tl, 0, sizeof(tl));
-  build_tiling(tl, host_shapes, L, Lq, S, TH, TW);
-  dim3 grid((unsigned)(tl.n_tiles * M), (unsigned)N);
-  if (N > 65535) return VLLM_EUNSUPPORTED;
-  if (L == 4 && P == 4)
-    msda_fwd_pair_kernel<TH, TW, NW, 16, 4, OutT><<<grid, NW * 32, 0, st>>>(pairs, shapes, lsi, loc, attw, out, S, M, L,
-                                                                            Lq, P, tl);
-  else
-    msda_fwd_pair_kernel<TH, TW, NW, 0, 0, OutT><<<grid, NW * 32, 0, st>>>(pairs, shapes, lsi, loc, attw, out, S, M, L,
-                                                                           Lq, P, tl);
-  VLLM_CHECK_LAUNCH();
-  return VLLM_OK;
-}
-
 template <typename T>
 static int launch_strict(const T* value, const int64_t* shapes, const int64_t* lsi, const T* loc, const T* attw,
                          T* out, int N, int S, int M, int D, int L, int Lq, int P, cudaStream_t st) {
@@ -683,7 +475,12 @@ static int check_common(const void* value, const void* shapes, const void* lsi, 
 
 extern "C" {
 
-int vllm_msda_set_variant(int v) { g_msda_variant = v; return VLLM_OK; }
+int vllm_msda_set_variant(int v) {
+  if (v != VLLM_MSDA_DEFAULT && v != VLLM_MSDA_NO_HINT && v != VLLM_MSDA_BF16_NO_WINDOW && v != VLLM_MSDA_FP32_WINDOW)
+    return VLLM_EINVAL;
+  g_msda_variant = v;
+  return VLLM_OK;
+}
 
 int vllm_msda_forward_f32(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
                           const float* sampling_loc, const float* attn_weight, float* out, int batch,
@@ -698,40 +495,26 @@ int vllm_msda_forward_f32(const float* value, const int64_t* spatial_shapes, con
   const int K = num_levels * num_point;
   if (!strict && channels == 32 && K <= 32 && vllm_aligned(value, 16) && vllm_aligned(out, 16) &&
       vllm_aligned(sampling_loc, 8)) {
-    // encoder shape, fp32 rows: the TMA-staged window kernel (msda_win.cu) is opt-in (variant 33) -- 128-byte rows leave
-    // room for an 8 x 8 patch only (not re-measured on the H100 against the global-memory patch kernel below);
-    // bf16 rows (vllm_msda_forward_bf16v) take the window kernel by default
-    if (g_msda_variant == 33) {
+    // encoder shape, fp32 rows: the TMA-staged window kernel (msda_win.cu) is opt-in -- 128-byte rows leave room for an
+    // 8 x 8 patch only (not re-measured on the H100 against the global-memory patch kernel below); bf16 rows
+    // (vllm_msda_forward_bf16v) take the window kernel by default
+    if (g_msda_variant == VLLM_MSDA_FP32_WINDOW) {
       const int r = msda_launch_window<float, float>(value, level_start_index, sampling_loc, attn_weight, out, batch,
                                                      spatial_size, num_heads, num_levels, num_query, num_point,
                                                      host_shapes_hint, st);
       if (r != 1) return r;
     }
-    switch (g_msda_variant) {
-      case 1: return launch_warp<8, 8, 8, float>(value, spatial_shapes, level_start_index, sampling_loc,
-                                                 attn_weight, out, batch, spatial_size, num_heads, num_levels,
-                                                 num_query, num_point, host_shapes_hint, st);
-      case 2: return launch_warp<16, 16, 16, float>(value, spatial_shapes, level_start_index, sampling_loc,
-                                                    attn_weight, out, batch, spatial_size, num_heads, num_levels,
-                                                    num_query, num_point, host_shapes_hint, st);
-      case 3: return launch_warp<16, 16, 32, float>(value, spatial_shapes, level_start_index, sampling_loc,
-                                                    attn_weight, out, batch, spatial_size, num_heads, num_levels,
-                                                    num_query, num_point, host_shapes_hint, st);
-      case 4: return launch_warp<8, 8, 8, float>(value, spatial_shapes, level_start_index, sampling_loc,
-                                                 attn_weight, out, batch, spatial_size, num_heads, num_levels,
-                                                 num_query, num_point, nullptr, st);
-      default:
-        // few queries (decoder: 100 / 900 object queries): 128-query tiles leave most SMs idle and make every warp
-        // walk 8 queries one HBM latency after the other -- 16-query tiles, 2 queries per warp, one pass
-        if (num_query != spatial_size &&
-            (long long)((num_query + 127) / 128) * num_heads * batch < 4ll * vllm_num_sms())
-          return launch_warp<4, 4, 8, float>(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, out,
-                                             batch, spatial_size, num_heads, num_levels, num_query, num_point, nullptr,
-                                             st);
-        return launch_warp<8, 16, 16, float>(value, spatial_shapes, level_start_index, sampling_loc,
-                                             attn_weight, out, batch, spatial_size, num_heads, num_levels,
-                                             num_query, num_point, host_shapes_hint, st);
-    }
+    if (g_msda_variant == VLLM_MSDA_NO_HINT) host_shapes_hint = nullptr;   // linear query tiles, as for a caller without one
+    // few queries (decoder: 100 / 900 object queries): 128-query tiles leave most SMs idle and make every warp
+    // walk 8 queries one HBM latency after the other -- 16-query tiles, 2 queries per warp, one pass
+    if (num_query != spatial_size &&
+        (long long)((num_query + 127) / 128) * num_heads * batch < 4ll * vllm_num_sms())
+      return launch_warp<4, 4, 8, float>(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, out,
+                                         batch, spatial_size, num_heads, num_levels, num_query, num_point, nullptr,
+                                         st);
+    return launch_warp<8, 16, 16, float>(value, spatial_shapes, level_start_index, sampling_loc,
+                                         attn_weight, out, batch, spatial_size, num_heads, num_levels,
+                                         num_query, num_point, host_shapes_hint, st);
   }
   return launch_strict<float>(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, out, batch,
                               spatial_size, num_heads, channels, num_levels, num_query, num_point, st);
@@ -749,7 +532,7 @@ int vllm_msda_forward_bf16v(const void* value, const int64_t* spatial_shapes, co
   if (!vllm_aligned(value, 16) || !vllm_aligned(out, 16) || !vllm_aligned(sampling_loc, 8)) return VLLM_EALIGN;
   cudaStream_t st = (cudaStream_t)stream;
   const __nv_bfloat16* v = (const __nv_bfloat16*)value;
-  if (g_msda_variant != 32) {                             // encoder shape: TMA-staged windows (msda_win.cu)
+  if (g_msda_variant != VLLM_MSDA_BF16_NO_WINDOW) {       // encoder shape: TMA-staged windows (msda_win.cu)
     const int r = out_bf16
         ? msda_launch_window<__nv_bfloat16, __nv_bfloat16>(v, level_start_index, sampling_loc, attn_weight,
                                                            (__nv_bfloat16*)out, batch, spatial_size, num_heads,
@@ -777,48 +560,6 @@ int vllm_msda_forward_bf16v(const void* value, const int64_t* spatial_shapes, co
   return launch_warp<8, 16, 16, float, __nv_bfloat16>(v, spatial_shapes, level_start_index, sampling_loc, attn_weight,
                                                       (float*)out, batch, spatial_size, num_heads, num_levels,
                                                       num_query, num_point, host_shapes_hint, st);
-}
-
-int vllm_msda_pack_pairs_bf16(const void* value, void* pairs, const int64_t* spatial_shapes,
-                              const int64_t* level_start_index, int batch, int spatial_size, int num_heads,
-                              int channels, int num_levels, void* stream) {
-  if (batch < 0 || spatial_size < 0 || num_heads <= 0 || num_levels <= 0) return VLLM_EINVAL;
-  if (channels != 32 || num_levels > MSDA_MAX_LEVELS) return VLLM_EUNSUPPORTED;
-  const long long n_chunks = (long long)batch * spatial_size * num_heads * 8;
-  if (n_chunks == 0) return VLLM_OK;
-  if (!value || !pairs || !spatial_shapes || !level_start_index) return VLLM_EINVAL;
-  if (!vllm_aligned(value, 16) || !vllm_aligned(pairs, 16)) return VLLM_EALIGN;
-  long long blocks = (n_chunks + 255) / 256;
-  const long long cap = (long long)vllm_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  msda_pack_pairs_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)value, (__nv_bfloat16*)pairs, n_chunks, spatial_shapes, level_start_index, spatial_size,
-      num_heads, num_levels);
-  VLLM_CHECK_LAUNCH();
-  return VLLM_OK;
-}
-
-int vllm_msda_forward_pairs(const void* pairs, const int64_t* spatial_shapes, const int64_t* level_start_index,
-                            const float* sampling_loc, const float* attn_weight, void* out, int out_bf16, int batch,
-                            int spatial_size, int num_heads, int channels, int num_levels, int num_query,
-                            int num_point, const int64_t* host_shapes_hint, void* stream) {
-  int rc = check_common(pairs, spatial_shapes, level_start_index, sampling_loc, attn_weight, out, batch,
-                        spatial_size, num_heads, channels, num_levels, num_query, num_point);
-  if (rc == 1000) return VLLM_OK;
-  if (rc) return rc;
-  const int K = num_levels * num_point;
-  if (channels != 32 || K > 32 || (K & 1)) return VLLM_EUNSUPPORTED;
-  if (((long long)batch * spatial_size * num_heads + 1) * 128 > INT_MAX) return VLLM_EUNSUPPORTED;  // zero line offset is int32
-  if (!vllm_aligned(pairs, 128) || !vllm_aligned(sampling_loc, 8)) return VLLM_EALIGN;
-  cudaStream_t st = (cudaStream_t)stream;
-  const __nv_bfloat16* v = (const __nv_bfloat16*)pairs;
-  if (out_bf16)
-    return launch_pair<8, 16, 16, __nv_bfloat16>(v, spatial_shapes, level_start_index, sampling_loc, attn_weight,
-                                                 (__nv_bfloat16*)out, batch, spatial_size, num_heads, num_levels,
-                                                 num_query, num_point, host_shapes_hint, st);
-  return launch_pair<8, 16, 16, float>(v, spatial_shapes, level_start_index, sampling_loc, attn_weight, (float*)out,
-                                       batch, spatial_size, num_heads, num_levels, num_query, num_point,
-                                       host_shapes_hint, st);
 }
 
 int vllm_msda_forward_f64(const double* value, const int64_t* spatial_shapes, const int64_t* level_start_index,

@@ -117,14 +117,7 @@ class GroundingDinoMultiscaleDeformableAttention(nn.Module):
             raise ValueError(f"Last dim of reference_points must be 2 or 4, but got {reference_points.shape[-1]}")
         # the reference upcasts value / weights to fp32 for its fp32-only kernel (:764-766); locations follow type
         # promotion.  With a bf16 value we read it in place (exact upcast inside the kernel) and write bf16 directly.
-        if (value.dtype == torch.bfloat16 and msda_ext.PAIRS_FOR_DENSE_QUERIES and 2 * Lq >= S
-                and msda_ext.supports_pairs(D, L, P)):
-            # many queries per value pixel (encoder self-attention): one pack pass buys two line fetches per sample
-            pairs = msda_ext.ms_deform_attn_pack_pairs(value.view(B, S, M, D), spatial_shapes, level_start_index)
-            out = msda_ext.ms_deform_attn_forward_pairs(pairs, spatial_shapes, level_start_index,
-                                                        loc.float().contiguous(), attention_weights.float().contiguous(),
-                                                        self.output_proj.weight.dtype)
-        elif value.dtype == torch.bfloat16 and msda_ext.supports_bf16_value(D, L, P):
+        if value.dtype == torch.bfloat16 and msda_ext.supports_bf16_value(D, L, P):
             out = msda_ext.ms_deform_attn_forward_bf16(value.view(B, S, M, D), spatial_shapes, level_start_index,
                                                        loc.float().contiguous(), attention_weights.float().contiguous(),
                                                        self.output_proj.weight.dtype)

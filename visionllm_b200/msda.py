@@ -60,7 +60,10 @@ def _host_shapes(spatial_shapes):
     return hit
 
 
-def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step):
+def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, im2col_step=None, *,
+                  value_dtypes=(torch.float32, torch.float64), loc_dtype=None, dtype_msg=None):
+    """loc_dtype None: sampling_loc / attn_weight must have the dtype of value (the reference's rule); else they must be
+    loc_dtype and a mismatch raises dtype_msg.  im2col_step None: the entry point has no such argument."""
     names = ("value", "spatial_shapes", "level_start_index", "sampling_loc", "attn_weight")
     for n, t in zip(names, (value, spatial_shapes, level_start_index, sampling_loc, attn_weight)):
         if not t.is_contiguous():
@@ -69,9 +72,12 @@ def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_w
             raise RuntimeError(f"{n} must be a CUDA tensor")
     if spatial_shapes.dtype != torch.int64 or level_start_index.dtype != torch.int64:
         raise RuntimeError("spatial_shapes / level_start_index must be int64")
-    if value.dtype not in (torch.float32, torch.float64):
+    if loc_dtype is not None:
+        if value.dtype not in value_dtypes or sampling_loc.dtype != loc_dtype or attn_weight.dtype != loc_dtype:
+            raise RuntimeError(dtype_msg)
+    elif value.dtype not in value_dtypes:
         raise RuntimeError(f"ms_deform_attn_forward not implemented for '{value.dtype}'")
-    if sampling_loc.dtype != value.dtype or attn_weight.dtype != value.dtype:
+    elif sampling_loc.dtype != value.dtype or attn_weight.dtype != value.dtype:
         raise RuntimeError("expected sampling_loc / attn_weight to have the dtype of value")
     if value.dim() != 4 or sampling_loc.dim() != 6 or attn_weight.dim() != 5:
         raise RuntimeError("expected value[N,S,M,D], sampling_loc[N,Lq,M,L,P,2], attn_weight[N,Lq,M,L,P]")
@@ -80,9 +86,10 @@ def _check_inputs(value, spatial_shapes, level_start_index, sampling_loc, attn_w
     _, Lq, M2, L2, P, two = sampling_loc.shape
     if (M2, L2, two) != (M, L, 2) or tuple(attn_weight.shape) != (N, Lq, M, L, P) or sampling_loc.shape[0] != N:
         raise RuntimeError("inconsistent MSDA shapes")
-    step = min(N, int(im2col_step)) if N > 0 else 1
-    if step <= 0 or (N > 0 and N % step != 0):
-        raise RuntimeError(f"batch({N}) must divide im2col_step({step})")
+    if im2col_step is not None:
+        step = min(N, int(im2col_step)) if N > 0 else 1
+        if step <= 0 or (N > 0 and N % step != 0):
+            raise RuntimeError(f"batch({N}) must divide im2col_step({step})")
     return N, S, M, D, L, Lq, P
 
 
@@ -128,23 +135,10 @@ def ms_deform_attn_forward_bf16(value, spatial_shapes, level_start_index, sampli
     """"Fast mode" (SURVEY 8d cfg 2b), an extension next to the reference API: value bf16 [N,S,M,32] read in place
     (the reference upcasts it with .float() first, gd.py:764), sampling_loc / attn_weight fp32, fp32 accumulation,
     out bf16 (default) or fp32.  Equal to ms_deform_attn_forward(value.float(), ...) up to the output rounding."""
-    for n, t in (("value", value), ("spatial_shapes", spatial_shapes), ("level_start_index", level_start_index),
-                 ("sampling_loc", sampling_loc), ("attn_weight", attn_weight)):
-        if not t.is_contiguous():
-            raise RuntimeError(f"{n} tensor has to be contiguous")
-        if not t.is_cuda:
-            raise RuntimeError(f"{n} must be a CUDA tensor")
-    if value.dtype != torch.bfloat16 or sampling_loc.dtype != torch.float32 or attn_weight.dtype != torch.float32:
-        raise RuntimeError("ms_deform_attn_forward_bf16: value must be bf16, sampling_loc / attn_weight fp32")
-    if spatial_shapes.dtype != torch.int64 or level_start_index.dtype != torch.int64:
-        raise RuntimeError("spatial_shapes / level_start_index must be int64")
-    if value.dim() != 4 or sampling_loc.dim() != 6 or attn_weight.dim() != 5:
-        raise RuntimeError("expected value[N,S,M,D], sampling_loc[N,Lq,M,L,P,2], attn_weight[N,Lq,M,L,P]")
-    N, S, M, D = value.shape
-    L = spatial_shapes.shape[0]
-    _, Lq, M2, L2, P, two = sampling_loc.shape
-    if (M2, L2, two) != (M, L, 2) or tuple(attn_weight.shape) != (N, Lq, M, L, P) or sampling_loc.shape[0] != N:
-        raise RuntimeError("inconsistent MSDA shapes")
+    N, S, M, D, L, Lq, P = _check_inputs(
+        value, spatial_shapes, level_start_index, sampling_loc, attn_weight, value_dtypes=(torch.bfloat16,),
+        loc_dtype=torch.float32,
+        dtype_msg="ms_deform_attn_forward_bf16: value must be bf16, sampling_loc / attn_weight fp32")
     out_dtype = out_dtype or torch.bfloat16
     if out_dtype not in (torch.bfloat16, torch.float32):
         raise RuntimeError("out_dtype must be bf16 or fp32")
@@ -193,79 +187,6 @@ def ms_deform_attn_forward_fused(value, spatial_shapes, level_start_index, qp, r
         return None
     _lib.check(rc, "ms_deform_attn_forward_fused")
     return out, attw
-
-
-# GDINO module policy (gdino.py): use the paired-row layout when the queries are (about) as many as the value pixels.
-PAIRS_FOR_DENSE_QUERIES = False
-
-
-def ms_deform_attn_pack_pairs(value, spatial_shapes, level_start_index):
-    """bf16 value [N,S,M,32] -> paired rows [N*S*M + 1, 2, 32] (pixel-major like value): slot 0 = value(s), slot 1 = value(s+1) when pixel s+1 is in
-    the same image row (else 0), so both horizontal corners of a bilinear sample sit in one aligned 128-byte line
-    (csrc/msda.cu, "paired-row fast mode").  One HBM pass: S*M*64 B read, S*M*128 B written per image.  The level
-    geometry is read on the device (no host copy, graph-capturable)."""
-    if value.dtype != torch.bfloat16 or not value.is_cuda or not value.is_contiguous() or value.dim() != 4:
-        raise RuntimeError("ms_deform_attn_pack_pairs: value must be a contiguous CUDA bf16 [N,S,M,D] tensor")
-    N, S, M, D = value.shape
-    if D != 32:
-        raise RuntimeError("ms_deform_attn_pack_pairs: D must be 32")
-    for t in (spatial_shapes, level_start_index):
-        if t.dtype != torch.int64 or not t.is_cuda or not t.is_contiguous():
-            raise RuntimeError("spatial_shapes / level_start_index must be contiguous CUDA int64 tensors")
-    if spatial_shapes.dim() != 2 or level_start_index.numel() != spatial_shapes.shape[0]:
-        raise RuntimeError("expected spatial_shapes[L,2] and level_start_index[L]")
-    pairs = torch.empty((N * S * M + 1, 2, D), dtype=torch.bfloat16, device=value.device)   # + the all-zero line
-    pairs._b200_value_shape = (N, S, M, D)
-    if N * S * M:
-        with torch.cuda.device(value.device):
-            rc = _lib.lib().vllm_msda_pack_pairs_bf16(value.data_ptr(), pairs.data_ptr(), spatial_shapes.data_ptr(),
-                                                      level_start_index.data_ptr(), N, S, M, D,
-                                                      spatial_shapes.shape[0], torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "ms_deform_attn_pack_pairs")
-    return pairs
-
-
-def ms_deform_attn_forward_pairs(pairs, spatial_shapes, level_start_index, sampling_loc, attn_weight, out_dtype=None):
-    """MSDA forward on the paired-row value tensor of `ms_deform_attn_pack_pairs` (same results as
-    ms_deform_attn_forward_bf16 up to fp32 summation order): two 128-byte line fetches per sample instead of four."""
-    for n, t in (("pairs", pairs), ("spatial_shapes", spatial_shapes), ("level_start_index", level_start_index),
-                 ("sampling_loc", sampling_loc), ("attn_weight", attn_weight)):
-        if not t.is_contiguous() or not t.is_cuda:
-            raise RuntimeError(f"{n} must be a contiguous CUDA tensor")
-    vs = getattr(pairs, "_b200_value_shape", None)
-    if pairs.dtype != torch.bfloat16 or pairs.dim() != 3 or pairs.shape[1] != 2 or vs is None:
-        raise RuntimeError("pairs must be the tensor returned by ms_deform_attn_pack_pairs")
-    if sampling_loc.dtype != torch.float32 or attn_weight.dtype != torch.float32:
-        raise RuntimeError("sampling_loc / attn_weight must be fp32")
-    if spatial_shapes.dtype != torch.int64 or level_start_index.dtype != torch.int64:
-        raise RuntimeError("spatial_shapes / level_start_index must be int64")
-    N, S, M, D = vs
-    if pairs.shape[0] != N * S * M + 1 or pairs.shape[2] != D:
-        raise RuntimeError("pairs does not match its recorded value shape")
-    L = spatial_shapes.shape[0]
-    if sampling_loc.dim() != 6 or attn_weight.dim() != 5:
-        raise RuntimeError("expected sampling_loc[N,Lq,M,L,P,2], attn_weight[N,Lq,M,L,P]")
-    _, Lq, M2, L2, P, two = sampling_loc.shape
-    if (M2, L2, two) != (M, L, 2) or tuple(attn_weight.shape) != (N, Lq, M, L, P) or sampling_loc.shape[0] != N:
-        raise RuntimeError("inconsistent MSDA shapes")
-    out_dtype = out_dtype or torch.bfloat16
-    if out_dtype not in (torch.bfloat16, torch.float32):
-        raise RuntimeError("out_dtype must be bf16 or fp32")
-    out = torch.empty((N, Lq, M * D), dtype=out_dtype, device=pairs.device)
-    if out.numel() == 0:
-        return out
-    hs = _host_shapes(spatial_shapes)
-    with torch.cuda.device(pairs.device):
-        rc = _lib.lib().vllm_msda_forward_pairs(
-            pairs.data_ptr(), spatial_shapes.data_ptr(), level_start_index.data_ptr(), sampling_loc.data_ptr(),
-            attn_weight.data_ptr(), out.data_ptr(), 1 if out_dtype == torch.bfloat16 else 0, N, S, M, D, L, Lq, P,
-            hs.data_ptr(), torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, "ms_deform_attn_forward_pairs")
-    return out
-
-
-def supports_pairs(D, L, P):
-    return D == 32 and L * P <= 32 and (L * P) % 2 == 0
 
 
 def supports_bf16_value(D, L, P):
