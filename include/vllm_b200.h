@@ -284,14 +284,14 @@ int vllm_rope_bf16(void* x, long long ld, const void* cos, const void* sin, long
  * (nn.MultiheadAttention / GroundingDinoBiMultiHeadAttention semantics, inverted).
  * attn_mask (uint8 [batch*heads, Tq, Tk], may be NULL): 1 = attend; exactly the [N*H, L, S] tensor
  * nn.MultiheadAttention receives as `attn_mask` (inverted), indexed by batch*heads + head.
- * causal != 0: query i sees keys <= i + (Tk - Tq).  head_dim in {32, 64, 128, 256}.
- * workspace (may be NULL): caller-owned scratch of workspace_bytes; when the query side alone cannot fill the
  * attn_bias (fp32 [bias_batches, heads, Tq, Tk], may be NULL): added to the scaled scores before the softmax;
  * batch b reads slab b % bias_batches -- Swin's relative-position bias (+ shifted-window mask, one slab per window
  * of an image; HF modeling_swin.py SwinSelfAttention.forward, used by the reference through AutoBackbone,
  * modeling_ov_grounding_dino_mask_dn.py:471-504).
+ * causal != 0: query i sees keys <= i + (Tk - Tq).  head_dim in {32, 64, 128, 256}.
+ * workspace (may be NULL): caller-owned scratch of workspace_bytes; when the query side alone cannot fill the
  * GPU (few queries, many keys: GDINO text->vision attention, 80 x 21760) the key axis is split across CTAs and
- * the partials (unnormalised O, running max, sum) are merged by a second kernel -- never needed for results. */
+ * the partials (unnormalised O, running max, sum) are merged by a second kernel.  NULL only turns the split off. */
 int vllm_attention_bf16(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk,
                         int heads, int kv_heads, int head_dim, long long q_batch_pitch,
                         long long q_token_pitch, long long k_batch_pitch, long long k_token_pitch,
@@ -314,8 +314,14 @@ int vllm_attention_bf16_tiles(const void* q, const void* k, const void* v, void*
                               long long o_token_pitch, const int* seqlens, const unsigned char* key_mask,
                               const unsigned char* attn_mask, float scale, const int* tile_counts,
                               const int* tile_lists, void* stream);
-/* Tuning knob (process-global), head_dim 128 / 256 without attn_mask / attn_bias: 0 = wgmma kernel (default),
- * 1 = warp-MMA kernel always. */
+/* Kernel selection for tests and benchmarks (process-global):
+ *   VLLM_ATTN_DEFAULT   the first kernel that takes the call: the wgmma kernel (head_dim 128 / 256 without attn_mask /
+ *                       attn_bias), the one-warp-per-window Swin kernel (head_dim 32, attn_bias only, no seqlens, not
+ *                       causal, Tq == Tk <= 64, kv_heads == heads), else the warp-MMA kernel
+ *   VLLM_ATTN_WARP_MMA  switches off the wgmma kernel and the window kernel: every call runs on the warp-MMA kernel
+ * Any other value: VLLM_EINVAL, nothing changes. */
+#define VLLM_ATTN_DEFAULT 0
+#define VLLM_ATTN_WARP_MMA 1
 int vllm_attention_set_variant(int variant);
 
 /* ---- tensor-parallel LLM decoder over peer memory (BASELINE cfg 5, SURVEY 8e) -------

@@ -4,6 +4,8 @@ Tolerance: bf16 P and bf16 output rounding -> |out - ref| <= 2^-7*|ref| + 2e-3*m
 import pytest
 import torch
 
+from visionllm_b200 import _lib
+
 pytestmark = pytest.mark.gpu
 
 
@@ -26,10 +28,9 @@ def ref_attn(q, k, v, causal, seqlens=None):
     return o
 
 
-@pytest.fixture(params=[0, 1], ids=["wgmma", "warp_mma"])
+@pytest.fixture(params=[_lib.ATTN_DEFAULT, _lib.ATTN_WARP_MMA], ids=["wgmma", "warp_mma"])
 def variant(request):
     """Run every case on the wgmma kernel (head_dim 128 / 256) and on the warp-MMA kernel."""
-    from visionllm_b200 import _lib
     with _lib.knob("attention_set_variant", request.param):
         yield request.param
 
@@ -159,7 +160,7 @@ def test_attention_wgmma_key_mask_and_split_kv(D, Tq, Tk):
     GDINO bi-attention's two shapes (many vision queries x 80 text keys; 80 text queries x thousands of vision keys,
     split along the key axis) with arbitrary key masks -- fully masked 64-key tiles,
     a batch entry whose mask leaves a single key.  Checked against fp32 torch and against the warp-MMA kernel."""
-    from visionllm_b200 import _lib, ops
+    from visionllm_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(D + Tq + Tk)
     B, H = 3, 4
     q = torch.randn(B, Tq, H, D, device="cuda", generator=g).bfloat16()
@@ -178,7 +179,7 @@ def test_attention_wgmma_key_mask_and_split_kv(D, Tq, Tk):
             s_ = s_.masked_fill(~mask[:, None, None, :], float("-inf"))
         ref = (torch.softmax(s_, -1) @ v.float().permute(0, 2, 1, 3)).permute(0, 2, 1, 3).reshape(B, Tq, H * D)
         check(out, ref)
-        with _lib.knob("attention_set_variant", 1):
+        with _lib.knob("attention_set_variant", _lib.ATTN_WARP_MMA):
             warp = ops.attention(q, k, v, key_mask=mask)
         check(out, warp.float())
 

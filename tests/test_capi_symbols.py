@@ -35,8 +35,8 @@ def test_python_binding_covers_the_header():
     assert set(declared_symbols()) == set(_lib.exported_symbols())
     # the named knob values are the header's
     src = open(os.path.join(ROOT, "include", "vllm_b200.h")).read()
-    defines = {k: int(v) for k, v in re.findall(r"#define VLLM_((?:MSDA|GEMM)_[A-Z0-9_]+) (\d+)", src) if k != "MSDA_STRICT"}
-    assert defines and defines == {k: getattr(_lib, k) for k in dir(_lib) if k.startswith(("MSDA_", "GEMM_"))}
+    defines = {k: int(v) for k, v in re.findall(r"#define VLLM_((?:MSDA|GEMM|ATTN)_[A-Z0-9_]+) (\d+)", src) if k != "MSDA_STRICT"}
+    assert defines and defines == {k: getattr(_lib, k) for k in dir(_lib) if k.startswith(("MSDA_", "GEMM_", "ATTN_"))}
 
 
 def test_version_string():
@@ -50,6 +50,7 @@ def test_round2_entry_points_marshal_and_accept_empty_problems():
     assert L.vllm_msda_set_window(0, 0, 0) == 0 and L.vllm_msda_set_window(-1, 0, 0) < 0
     assert L.vllm_msda_set_variant(_lib.MSDA_DEFAULT) == 0 and L.vllm_msda_set_variant(1) < 0      # not a named value
     assert L.vllm_gemm_set_variant(_lib.GEMM_DEFAULT) == 0 and L.vllm_gemm_set_variant(1) < 0
+    assert L.vllm_attention_set_variant(_lib.ATTN_DEFAULT) == 0 and L.vllm_attention_set_variant(2) < 0
     with pytest.raises(_lib.VllmB200Error):                                                          # a rejected value must not
         with _lib.knob("msda_set_variant", 1):                                                       # silently test the default path
             pass

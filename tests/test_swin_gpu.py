@@ -64,12 +64,12 @@ def test_attention_additive_bias(T, H, D, nB):
     if D == 32 and T <= 64:
         # r2: these calls take the one-warp-per-(window, head) kernel; same arithmetic order as the general kernel
         from visionllm_b200 import _lib
-        with _lib.knob("attention_set_variant", 1):
+        with _lib.knob("attention_set_variant", _lib.ATTN_WARP_MMA):
             general = ops.attention(q, k, v, attn_bias=bias.contiguous())
         assert torch.equal(out, general)
         qkv = torch.randn(B, T, 3, H, D, device="cuda", generator=g).bfloat16()          # packed, strided views like swin.py
         o1 = ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], attn_bias=bias.contiguous())
-        with _lib.knob("attention_set_variant", 1):
+        with _lib.knob("attention_set_variant", _lib.ATTN_WARP_MMA):
             o2 = ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], attn_bias=bias.contiguous())
         assert torch.equal(o1, o2)
     with pytest.raises(RuntimeError):

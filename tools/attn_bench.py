@@ -28,7 +28,7 @@ for name, (B, T, H, causal) in SHAPES.items():
     q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
     fl = 4.0 * B * H * T * T * 128 * (0.5 if causal else 1.0)
     r = {}
-    for var, nm in ((0, "wgmma"), (1, "warp_mma")):
+    for var, nm in ((_lib.ATTN_DEFAULT, "wgmma"), (_lib.ATTN_WARP_MMA, "warp_mma")):
         try:
             with _lib.knob("attention_set_variant", var):
                 ms = timeit(lambda: ops.attention(q, k, v, causal=causal))

@@ -93,13 +93,14 @@ _SIGNATURES = {
 }
 
 
-# values of vllm_msda_set_variant / vllm_gemm_set_variant (include/vllm_b200.h)
+# values of vllm_msda_set_variant / vllm_gemm_set_variant / vllm_attention_set_variant (include/vllm_b200.h)
 MSDA_DEFAULT, MSDA_NO_HINT, MSDA_BF16_NO_WINDOW, MSDA_FP32_WINDOW = 0, 4, 32, 33
 GEMM_DEFAULT, GEMM_WIDE_TILE = 0, 2
+ATTN_DEFAULT, ATTN_WARP_MMA = 0, 1
 
 # the process-global path / tuning setters and the arguments that restore the library's own choice
 _KNOB_DEFAULTS = {"msda_set_variant": (MSDA_DEFAULT,), "msda_set_window": (0, 0, 0), "msda_set_window_fill": (-1,),
-                  "gemm_set_variant": (GEMM_DEFAULT,), "attention_set_variant": (0,)}
+                  "gemm_set_variant": (GEMM_DEFAULT,), "attention_set_variant": (ATTN_DEFAULT,)}
 
 
 class VllmB200Error(RuntimeError):

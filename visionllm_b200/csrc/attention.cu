@@ -17,33 +17,12 @@
 // packed qkv GEMM output is consumed in place; o is [batch, tokens, heads*D].  seqlens (optional, int32
 // [batch]) masks keys >= len (right padding / key_padding_mask); every query row is computed (rows of
 // padded queries hold finite don't-care values, as in the reference).
-#include "common.cuh"
+#include "attention.cuh"
+#include "vllm_b200.h"   // VLLM_ATTN_* variant names
 
 namespace {
 
 constexpr int BM = 64, NW = 4;
-
-struct AttnArgs {
-  const __nv_bfloat16 *q, *k, *v;
-  __nv_bfloat16* o;
-  long long q_bs, k_bs, v_bs, o_bs;  // batch pitches
-  long long q_ts, k_ts, v_ts, o_ts;  // token pitches
-  const int* seqlens;
-  const unsigned char* key_mask;   // optional [batch, Tk], 1 = attend (arbitrary key_padding_mask)
-  const unsigned char* attn_mask;  // optional [batch*heads, Tq, Tk], 1 = attend (nn.MultiheadAttention attn_mask, inverted)
-  const float* attn_bias;          // optional additive bias [bias_batches, heads, Tq, Tk] fp32; batch b reads slab b % bias_batches
-  int bias_batches;
-  int Tq, Tk, heads, kv_heads, causal;
-  float scale_log2;
-  int n_splits;      // split-KV: CTAs along the key axis per query block (1 = off)
-  float* ws;         // workspace [batch*heads*n_splits*Tq][D + 2] fp32 partials (unnormalised O, m, l)
-  // Live-tile lists of a sparse attn_mask (vllm_attention_mask_tiles): per (batch*heads, 64-row query block) the ascending
-  // ids of the 64-key tiles holding at least one allowed pair.  A fully blocked tile leaves the online softmax untouched
-  // (all scores -inf: corr = 1, p = 0), so walking only the live tiles gives bit-identical results.
-  const int* tile_counts;   // [batch*heads, q_blocks] or nullptr
-  const int* tile_lists;    // [batch*heads, q_blocks, k_tiles]
-  int q_blocks, k_tiles;
-};
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool pred) {
   const int sz = pred ? 16 : 0;
@@ -504,12 +483,8 @@ window_attn_kernel(const WinArgs a) {
 
 static int launch_window(const AttnArgs& a, int batch, cudaStream_t st) {
   constexpr int SMEM = 4 * 3 * 64 * 32 * 2;               // 4 warps x (Q, K, V) x 64 rows x 64 B
-  static bool set = false;
-  if (!set) {
-    cudaError_t e = cudaFuncSetAttribute(window_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return (int)e;
-    set = true;
-  }
+  const cudaError_t e = vllm_smem_optin(window_attn_kernel, SMEM);
+  if (e != cudaSuccess) return (int)e;
   WinArgs w;
   w.q = a.q; w.k = a.k; w.v = a.v; w.o = a.o;
   w.q_bs = a.q_bs; w.k_bs = a.k_bs; w.v_bs = a.v_bs; w.o_bs = a.o_bs;
@@ -524,94 +499,82 @@ static int launch_window(const AttnArgs& a, int batch, cudaStream_t st) {
   return VLLM_OK;
 }
 
+// Split-KV: when the query tiles alone cannot fill the GPU (e.g. 80 text queries over 21760 pixels), several CTAs share one
+// query tile along the key axis, write unnormalised partials to the workspace, and splitkv_combine_kernel merges them.
+// The constants of one kernel family:
+struct SplitKv {
+  int q_tile, k_tile;   // query rows / keys per tile
+  int per_sm;           // resident CTAs per SM
+  int tiles_per_split;  // largest split count = min(key tiles / tiles_per_split, 64)
+  int fixed_tiles;      // fixed cost of a CTA (Q load, prologue, partial write-out) in key tiles
+  bool reject_empty;    // skip counts that would leave the last split(s) without a key tile
+};
+
+// The split count (1 = none) that minimises (waves of resident CTAs) x (key tiles per split + fixed cost): a count that
+// spills a few CTAs into one more wave costs a whole extra pass.  The partials of a count must fit the workspace.
+static int split_kv_count(const AttnArgs& a, int batch, int D, const SplitKv& f, const void* workspace,
+                          long long workspace_bytes) {
+  const long long ctas = (long long)((a.Tq + f.q_tile - 1) / f.q_tile) * a.heads * batch;
+  const int n_tiles = (a.Tk + f.k_tile - 1) / f.k_tile;
+  if (!workspace || a.causal || a.tile_counts || ctas >= 2LL * vllm_num_sms() || n_tiles < 16) return 1;
+  const long long slots = (long long)vllm_num_sms() * f.per_sm;
+  long long best = 1, best_cost = (ctas + slots - 1) / slots * (n_tiles + f.fixed_tiles);
+  const long long max_s = n_tiles / f.tiles_per_split < 64 ? n_tiles / f.tiles_per_split : 64;
+  for (long long sp = 2; sp <= max_s; ++sp) {
+    if ((long long)batch * a.heads * sp * a.Tq * (D + 2) * 4 > workspace_bytes) break;
+    if (f.reject_empty && (sp - 1) * ((n_tiles + sp - 1) / sp) >= n_tiles) continue;
+    const long long waves = (ctas * sp + slots - 1) / slots;
+    const long long cost = waves * ((n_tiles + sp - 1) / sp + f.fixed_tiles);
+    if (cost < best_cost) { best_cost = cost; best = sp; }
+  }
+  return (int)best;
+}
+
+template <int D>
+static int launch_combine(const AttnArgs& a, int batch, cudaStream_t st) {
+  const long long n_rows = (long long)batch * a.heads * a.Tq;
+  splitkv_combine_kernel<D><<<(unsigned)((n_rows + 3) / 4), 128, 0, st>>>(a.ws, a.o, a.o_bs, a.o_ts, a.Tq, a.heads,
+                                                                         a.n_splits, n_rows);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
 template <int D, int BN = 64>
 int launch(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long workspace_bytes) {
   constexpr int SMEM = BM * D * 2 + 4 * BN * D * 2;
-  static bool set = false;
-  if (!set) {
-    cudaError_t e = cudaFuncSetAttribute(flash_fwd_kernel<D, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return (int)e;
-    set = true;
-  }
-  const int m_blocks = (a.Tq + BM - 1) / BM;
-  // split-KV when the query side alone cannot fill the machine (e.g. 80 text queries over 21760 pixels)
-  a.n_splits = 1; a.ws = nullptr;
-  const long long ctas = (long long)m_blocks * a.heads * batch;
-  const int n_tiles = (a.Tk + BN - 1) / BN;
-  if (workspace && !a.causal && !a.tile_counts && ctas < 2LL * vllm_num_sms() && n_tiles >= 16) {
-    // pick the split count that minimises (waves of resident CTAs) x (key tiles per split): a count that spills a
-    // few CTAs into one more wave costs a whole extra pass
-    static int per_sm = 0;
-    if (!per_sm) {
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, flash_fwd_kernel<D, BN>, NW * 32, SMEM) != cudaSuccess ||
-          per_sm < 1)
-        per_sm = 1;
-    }
-    const long long slots = (long long)vllm_num_sms() * per_sm;
-    long long best = 1, best_cost = (ctas + slots - 1) / slots * (n_tiles + 2);
-    const long long max_s = n_tiles / 8 < 64 ? n_tiles / 8 : 64;
-    for (long long sp = 2; sp <= max_s; ++sp) {
-      if ((long long)batch * a.heads * sp * a.Tq * (D + 2) * 4 > workspace_bytes) break;
-      const long long waves = (ctas * sp + slots - 1) / slots;
-      const long long cost = waves * ((n_tiles + sp - 1) / sp + 2);       // +2 tiles: prologue / partial write-out
-      if (cost < best_cost) { best_cost = cost; best = sp; }
-    }
-    if (best >= 2) { a.n_splits = (int)best; a.ws = (float*)workspace; }
-  }
-  dim3 grid((unsigned)(m_blocks * a.n_splits), a.heads, batch);
+  const cudaError_t e = vllm_smem_optin(flash_fwd_kernel<D, BN>, SMEM);
+  if (e != cudaSuccess) return (int)e;
+  static int per_sm = 0;                                  // depends on the kernel and the architecture only
+  if (!per_sm && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, flash_fwd_kernel<D, BN>, NW * 32, SMEM) != cudaSuccess ||
+                  per_sm < 1))
+    per_sm = 1;
+  a.n_splits = split_kv_count(a, batch, D, {BM, BN, per_sm, 8, 2, false}, workspace, workspace_bytes);
+  a.ws = a.n_splits > 1 ? (float*)workspace : nullptr;
+  dim3 grid((unsigned)(((a.Tq + BM - 1) / BM) * a.n_splits), a.heads, batch);
   flash_fwd_kernel<D, BN><<<grid, NW * 32, SMEM, st>>>(a);
   VLLM_CHECK_LAUNCH();
-  if (a.n_splits > 1) {
-    const long long n_rows = (long long)batch * a.heads * a.Tq;
-    splitkv_combine_kernel<D><<<(unsigned)((n_rows + 3) / 4), 128, 0, st>>>(a.ws, a.o, a.o_bs, a.o_ts, a.Tq, a.heads,
-                                                                           a.n_splits, n_rows);
-    VLLM_CHECK_LAUNCH();
-  }
-  return VLLM_OK;
+  return a.n_splits > 1 ? launch_combine<D>(a, batch, st) : VLLM_OK;
+}
+
+// The wgmma kernel (attention_wgmma.cu) runs one CTA of 128 query rows per SM.  An unmasked head_dim-128 call never
+// splits, and only this family rejects empty splits: both as tuned so far (the split-KV re-tune, DESIGN §10 item 3).
+template <int D>
+static int launch_wgmma(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long workspace_bytes) {
+  if (D == 128 && !a.key_mask) workspace = nullptr;
+  a.n_splits = split_kv_count(a, batch, D, {128, 64, 1, 4, 4, true}, workspace, workspace_bytes);
+  a.ws = a.n_splits > 1 ? (float*)workspace : nullptr;
+  const int rc = vllm_attention_wgmma(a, batch, D, st);
+  return rc == VLLM_OK && a.n_splits > 1 ? launch_combine<D>(a, batch, st) : rc;
 }
 
 }  // namespace
 
-int vllm_attention_wgmma(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
-                         int kv_heads, int head_dim, long long q_bs, long long q_ts, long long k_bs, long long k_ts,
-                         long long v_bs, long long v_ts, long long o_bs, long long o_ts, const int* seqlens,
-                         const unsigned char* key_mask, int causal, float scale, int n_splits, float* ws, cudaStream_t st);
-
-// wgmma path for head_dim 256 and for key-masked head_dim 128 calls: picks a split-KV count like launch<> above
-// when the query tiles alone cannot fill the SMs, then merges the partials with the same combine kernel.
-template <int D>
-static int launch_wgmma_split(const AttnArgs& a, int batch, float scale, cudaStream_t st, void* workspace,
-                              long long workspace_bytes) {
-  const int q_tiles = (a.Tq + 127) / 128;
-  const long long ctas = (long long)q_tiles * a.heads * batch;
-  const int n_tiles = (a.Tk + 63) / 64;
-  long long best = 1;
-  if (workspace && !a.causal && ctas < 2LL * vllm_num_sms() && n_tiles >= 16) {
-    const long long slots = vllm_num_sms();                               // one CTA per SM
-    long long best_cost = (ctas + slots - 1) / slots * (n_tiles + 4);
-    const long long max_s = n_tiles / 4 < 64 ? n_tiles / 4 : 64;
-    for (long long sp = 2; sp <= max_s; ++sp) {
-      if ((long long)batch * a.heads * sp * a.Tq * (D + 2) * 4 > workspace_bytes) break;
-      if ((sp - 1) * ((n_tiles + sp - 1) / sp) >= n_tiles) continue;      // the last split(s) would get no key tile at all
-      const long long waves = (ctas * sp + slots - 1) / slots;
-      const long long cost = waves * ((n_tiles + sp - 1) / sp + 4);       // +4 tiles: Q load, prologue, partial write-out
-      if (cost < best_cost) { best_cost = cost; best = sp; }
-    }
-  }
-  const int rc = vllm_attention_wgmma(a.q, a.k, a.v, a.o, batch, a.Tq, a.Tk, a.heads, a.kv_heads, D, a.q_bs, a.q_ts, a.k_bs,
-                                      a.k_ts, a.v_bs, a.v_ts, a.o_bs, a.o_ts, a.seqlens, a.key_mask, a.causal, scale,
-                                      (int)best, best > 1 ? (float*)workspace : nullptr, st);
-  if (rc != VLLM_OK || best == 1) return rc;
-  const long long n_rows = (long long)batch * a.heads * a.Tq;
-  splitkv_combine_kernel<D><<<(unsigned)((n_rows + 3) / 4), 128, 0, st>>>((const float*)workspace, a.o, a.o_bs, a.o_ts, a.Tq,
-                                                                         a.heads, (int)best, n_rows);
-  VLLM_CHECK_LAUNCH();
+static int g_attn_variant = VLLM_ATTN_DEFAULT;  // see vllm_attention_set_variant
+extern "C" int vllm_attention_set_variant(int v) {
+  if (v != VLLM_ATTN_DEFAULT && v != VLLM_ATTN_WARP_MMA) return VLLM_EINVAL;
+  g_attn_variant = v;
   return VLLM_OK;
 }
-
-// head_dim 128 / 256 without attn_mask / attn_bias: 0 = the wgmma kernel (attention_wgmma.cu), 1 = always the warp-MMA kernel.
-static int g_attn_variant = 0;
-extern "C" int vllm_attention_set_variant(int v) { g_attn_variant = v; return VLLM_OK; }
 
 static int attention_impl(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk,
                           int heads, int kv_heads, int head_dim, long long q_batch_pitch,
@@ -639,23 +602,22 @@ static int attention_impl(const void* q, const void* k, const void* v, void* o, 
   a.q_ts = q_token_pitch; a.k_ts = k_token_pitch; a.v_ts = v_token_pitch; a.o_ts = o_token_pitch;
   a.seqlens = seqlens; a.key_mask = key_mask; a.attn_mask = attn_mask; a.attn_bias = attn_bias; a.bias_batches = bias_batches; a.Tq = Tq; a.Tk = Tk; a.heads = heads; a.kv_heads = kv_heads; a.causal = causal;
   a.scale_log2 = scale * 1.4426950408889634f;
+  a.n_splits = 1; a.ws = nullptr;
   a.tile_counts = tile_counts; a.tile_lists = tile_lists; a.q_blocks = (Tq + 63) / 64; a.k_tiles = (Tk + 63) / 64;
   cudaStream_t st = (cudaStream_t)stream;
-  if (head_dim == 128 && g_attn_variant == 0 && !key_mask && !attn_mask && !attn_bias) {
-    const int rc = vllm_attention_wgmma(q, k, v, o, batch, Tq, Tk, heads, kv_heads, 128, q_batch_pitch, q_token_pitch,
-                                        k_batch_pitch, k_token_pitch, v_batch_pitch, v_token_pitch, o_batch_pitch,
-                                        o_token_pitch, seqlens, nullptr, causal, scale, 1, nullptr, st);
-    if (rc != VLLM_EUNSUPPORTED) return rc;   // views a TMA descriptor cannot express use the warp-MMA kernel
-  }
-  if ((head_dim == 256 || (head_dim == 128 && key_mask)) && g_attn_variant == 0 && !attn_mask && !attn_bias) {
-    const int rc = head_dim == 256 ? launch_wgmma_split<256>(a, batch, scale, st, workspace, workspace_bytes)
-                                   : launch_wgmma_split<128>(a, batch, scale, st, workspace, workspace_bytes);
+  // The first kernel that takes the call runs it; VLLM_ATTN_WARP_MMA leaves only the last one.
+  const bool all_kernels = g_attn_variant == VLLM_ATTN_DEFAULT;
+  // 1. wgmma: head_dim 128 / 256 without attn_mask / attn_bias; a view a TMA descriptor cannot express goes on to 3.
+  if (all_kernels && (head_dim == 128 || head_dim == 256) && !attn_mask && !attn_bias) {
+    const int rc = head_dim == 128 ? launch_wgmma<128>(a, batch, st, workspace, workspace_bytes)
+                                   : launch_wgmma<256>(a, batch, st, workspace, workspace_bytes);
     if (rc != VLLM_EUNSUPPORTED) return rc;
   }
-  // Swin windows: head_dim 32, one key tile, additive bias only -> one warp per (window, head) (variant 1 keeps the general kernel)
-  if (head_dim == 32 && g_attn_variant != 1 && attn_bias && !key_mask && !attn_mask && !seqlens && !causal && Tq == Tk && Tq <= 64 &&
+  // 2. Swin windows: head_dim 32, one key tile, additive bias only -> one warp per (window, head)
+  if (all_kernels && head_dim == 32 && attn_bias && !key_mask && !attn_mask && !seqlens && !causal && Tq == Tk && Tq <= 64 &&
       kv_heads == heads)
     return launch_window(a, batch, st);
+  // 3. the warp-MMA kernel
   switch (head_dim) {
     case 128: return launch<128>(a, batch, st, workspace, workspace_bytes);
     case 64: return launch<64>(a, batch, st, workspace, workspace_bytes);

@@ -15,7 +15,7 @@
 // [batch, Tk] (1 = attend: the text / vision padding masks of the bi-attention); n_splits > 1 lets several CTAs share one
 // query tile along the key axis (80 text queries over 21760 pixels) and write unnormalised partials in attention.cu's
 // split-KV workspace layout.
-#include "common.cuh"
+#include "attention.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -275,37 +275,25 @@ template <int D, bool KM>
 static int launch_wgmma(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const Args& a, int batch,
                         cudaStream_t st) {
   auto kern = attn_fwd_wgmma_kernel<D, KM>;
-  static bool attr_set[64] = {false};
-  bool* set = vllm_device_flag(attr_set);
-  if (!set || !*set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<D>::SMEM);
-    if (e != cudaSuccess) return (int)e;
-    if (set) *set = true;
-  }
+  const cudaError_t e = vllm_smem_optin(kern, Cfg<D>::SMEM);
+  if (e != cudaSuccess) return (int)e;
   dim3 grid((unsigned)(((a.Tq + BQ - 1) / BQ) * a.n_splits), a.heads, batch);
   kern<<<grid, THREADS, Cfg<D>::SMEM, st>>>(tq, tk, tv, a);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }
 
-// head_dim 128 / 256; key_mask optional ([batch, Tk] bytes, 1 = attend); n_splits > 1: partials go to `ws`
-// ([batch*heads*n_splits*Tq][head_dim + 2] fp32) and the caller merges them (attention.cu splitkv_combine_kernel).
-// VLLM_EUNSUPPORTED: views a TMA descriptor cannot express (the caller then uses the warp-MMA kernel).
-int vllm_attention_wgmma(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk, int heads,
-                         int kv_heads, int head_dim, long long q_bs, long long q_ts, long long k_bs, long long k_ts,
-                         long long v_bs, long long v_ts, long long o_bs, long long o_ts, const int* seqlens,
-                         const unsigned char* key_mask, int causal, float scale, int n_splits, float* ws, cudaStream_t st) {
+int vllm_attention_wgmma(const AttnArgs& at, int batch, int head_dim, cudaStream_t st) {
   if (head_dim != 128 && head_dim != 256) return VLLM_EUNSUPPORTED;
-  if (n_splits < 1 || (n_splits > 1 && (!ws || causal))) return VLLM_EINVAL;
   const uint64_t D = (uint64_t)head_dim;
   CUtensorMap tq, tk, tv;
-  if (make_tmap(&tq, q, (uint64_t)heads * D, Tq, batch, q_ts, q_bs, BQ)) return VLLM_EUNSUPPORTED;
-  if (make_tmap(&tk, k, (uint64_t)kv_heads * D, Tk, batch, k_ts, k_bs, BKV)) return VLLM_EUNSUPPORTED;
-  if (make_tmap(&tv, v, (uint64_t)kv_heads * D, Tk, batch, v_ts, v_bs, BKV)) return VLLM_EUNSUPPORTED;
+  if (make_tmap(&tq, at.q, (uint64_t)at.heads * D, at.Tq, batch, at.q_ts, at.q_bs, BQ)) return VLLM_EUNSUPPORTED;
+  if (make_tmap(&tk, at.k, (uint64_t)at.kv_heads * D, at.Tk, batch, at.k_ts, at.k_bs, BKV)) return VLLM_EUNSUPPORTED;
+  if (make_tmap(&tv, at.v, (uint64_t)at.kv_heads * D, at.Tk, batch, at.v_ts, at.v_bs, BKV)) return VLLM_EUNSUPPORTED;
   Args a;
-  a.o = (__nv_bfloat16*)o; a.o_bs = o_bs; a.o_ts = o_ts; a.seqlens = seqlens; a.Tq = Tq; a.Tk = Tk;
-  a.heads = heads; a.kv_heads = kv_heads; a.causal = causal; a.scale_log2 = scale * 1.4426950408889634f;
-  a.key_mask = key_mask; a.n_splits = n_splits; a.ws = ws;
-  if (head_dim == 128) return key_mask ? launch_wgmma<128, true>(tq, tk, tv, a, batch, st) : launch_wgmma<128, false>(tq, tk, tv, a, batch, st);
-  return key_mask ? launch_wgmma<256, true>(tq, tk, tv, a, batch, st) : launch_wgmma<256, false>(tq, tk, tv, a, batch, st);
+  a.o = at.o; a.o_bs = at.o_bs; a.o_ts = at.o_ts; a.seqlens = at.seqlens; a.Tq = at.Tq; a.Tk = at.Tk;
+  a.heads = at.heads; a.kv_heads = at.kv_heads; a.causal = at.causal; a.scale_log2 = at.scale_log2;
+  a.key_mask = at.key_mask; a.n_splits = at.n_splits; a.ws = at.ws;
+  if (head_dim == 128) return at.key_mask ? launch_wgmma<128, true>(tq, tk, tv, a, batch, st) : launch_wgmma<128, false>(tq, tk, tv, a, batch, st);
+  return at.key_mask ? launch_wgmma<256, true>(tq, tk, tv, a, batch, st) : launch_wgmma<256, false>(tq, tk, tv, a, batch, st);
 }

@@ -35,12 +35,13 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// Per-device one-time set-up (cudaFuncSetAttribute is a property of the function ON A DEVICE): the flag of the current
-// device in a caller-owned array, or nullptr when the device cannot be told (then the caller repeats the set-up).
-static inline bool* vllm_device_flag(bool (&flags)[64]) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  return &flags[dev];
+// Raises the dynamic shared-memory limit of kernel `kern` on the current device to at least `bytes`.  The limit is a
+// property of the function ON A DEVICE, so what was set is remembered per (device, kernel) and only a larger request
+// calls cudaFuncSetAttribute again (runtime.cu).
+cudaError_t vllm_smem_optin(const void* kern, int bytes);
+template <typename Kern>
+static inline cudaError_t vllm_smem_optin(Kern* kern, int bytes) {
+  return vllm_smem_optin(reinterpret_cast<const void*>(kern), bytes);
 }
 
 // Number of SMs of the current device (cached per process; H100 SXM = 132).

@@ -369,13 +369,8 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
   // Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so one wave of
   // CTAs covers a near-square patch of tiles (minimal A+B bytes per wave).
   g.group_m = 8;
-  static bool attr_set[64] = {false};
-  bool* set = vllm_device_flag(attr_set);
-  if (!set || !*set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, C_::SMEM);
-    if (e != cudaSuccess) return (int)e;
-    if (set) *set = true;
-  }
+  const cudaError_t e = vllm_smem_optin(gemm_bf16_wgmma_kernel<BN>, C_::SMEM);
+  if (e != cudaSuccess) return (int)e;
   gemm_bf16_wgmma_kernel<BN><<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, g);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;

@@ -576,13 +576,8 @@ int msda_launch_window(const ValT* value, const int64_t* lsi, const float* loc, 
   dim3 grid((unsigned)(e->wp.RX * e->wp.RY * M), (unsigned)N);
   const bool big = e->smem > 110 * 1024;                   // one 32-warp CTA per SM (tuning knob territory)
   auto launch = [&](auto kern, int nw) -> int {
-    static int configured = -1;
-    if (configured < e->smem) {
-      const int want = big ? e->smem : 112 * 1024;
-      cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, want);
-      if (err != cudaSuccess) return (int)err;
-      configured = want;
-    }
+    const cudaError_t err = vllm_smem_optin(kern, big ? e->smem : 112 * 1024);
+    if (err != cudaSuccess) return (int)err;
     MsdaWin wp = e->wp;
     set_fill(wp, (int)sizeof(ValT));
     kern<<<grid, nw * 32, e->smem, st>>>(e->maps, value, lsi, loc, attw, out, S, M, Lq, P, wp, MsdaQp{});
@@ -604,13 +599,8 @@ static int launch_window_qp(const __nv_bfloat16* value, const int64_t* lsi, cons
   dim3 grid((unsigned)(e->wp.RX * e->wp.RY * M), (unsigned)N);
   const bool big = e->smem > 110 * 1024;
   auto launch = [&](auto kern, int nw) -> int {
-    static int configured = -1;
-    if (configured < e->smem) {
-      const int want = big ? e->smem : 112 * 1024;
-      cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, want);
-      if (err != cudaSuccess) return (int)err;
-      configured = want;
-    }
+    const cudaError_t err = vllm_smem_optin(kern, big ? e->smem : 112 * 1024);
+    if (err != cudaSuccess) return (int)err;
     MsdaWin wp = e->wp;
     set_fill(wp, 2);
     kern<<<grid, nw * 32, e->smem, st>>>(e->maps, value, lsi, nullptr, nullptr, out, S, M, Lq, P, wp, fq);
