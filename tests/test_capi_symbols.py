@@ -39,6 +39,21 @@ def test_python_binding_covers_the_header():
     assert defines and defines == {k: getattr(_lib, k) for k in dir(_lib) if k.startswith(("MSDA_", "GEMM_", "ATTN_"))}
 
 
+def test_every_setter_has_a_knob_default():
+    """`_lib.knob` restores a process-global setter from `_KNOB_DEFAULTS`: every bound vllm_*_set_* needs an entry with
+    one value per argument, and the library must accept it (a setter without one would leak its value into every
+    later call)."""
+    setters = sorted(s[len("vllm_"):] for s in _lib._SIGNATURES if re.fullmatch(r"vllm_\w+_set_\w+", s))
+    assert "gemm_set_sm_limit" in setters
+    missing = [s for s in setters if s not in _lib._KNOB_DEFAULTS]
+    assert not missing, missing
+    L = _lib.lib()
+    for s in setters:
+        defaults = _lib._KNOB_DEFAULTS[s]
+        assert len(defaults) == len(_lib._SIGNATURES["vllm_" + s][1]), s
+        assert getattr(L, "vllm_" + s)(*defaults) == 0, s
+
+
 def test_version_string():
     assert b"sm_90a" in _lib.lib().vllm_version()
 

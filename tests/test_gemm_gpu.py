@@ -55,32 +55,8 @@ def test_gemm_plain(M, N, K, variant):
     close(out, ref)
 
 
-@pytest.mark.parametrize("variant", VARIANTS)
-@pytest.mark.parametrize("act", ["gelu", "relu", "silu", "quick_gelu", None])
-def test_gemm_epilogues(act, variant):
-    M, N, K = 520, 768, 320
-    x, w = mk(M, N, K, seed=3)
-    g = torch.Generator(device="cuda").manual_seed(9)
-    bias = torch.randn(N, device="cuda", generator=g).bfloat16()
-    ls = (torch.rand(N, device="cuda", generator=g) * 0.2).bfloat16()
-    res = torch.randn(M, N, device="cuda", generator=g).bfloat16()
-    with _lib.knob("gemm_set_variant", variant):
-        out = ops().linear(x, w, bias=bias, act=act, colscale=ls, residual=res)
-        out32 = ops().linear(x, w, bias=bias, act=act, out_dtype=torch.float32)
-    y = x.float() @ w.float().T + bias.float()
-    if act == "gelu":
-        y = torch.nn.functional.gelu(y)
-    elif act == "relu":
-        y = torch.relu(y)
-    elif act == "silu":
-        y = torch.nn.functional.silu(y)
-    elif act == "quick_gelu":
-        y = y * torch.sigmoid(1.702 * y)
-    assert out32.dtype == torch.float32
-    assert (out32 - y).abs().max() <= 1e-3 * y.abs().max()
-    close(out, y * ls.float() + res.float())
-
-
+# the fused epilogues (bias / activation / colscale / residual / row mask, fp32 and bf16 output) are checked against
+# fp64 in tests/test_gemm_epilogue_gpu.py
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_gemm_swiglu_interleaved(variant):
     M, I, K = 300, 1376, 512
@@ -117,6 +93,27 @@ def test_gemm_argument_errors():
         o.linear(x, w[:, :32])
     with pytest.raises(RuntimeError):
         o.linear(x[:, :36], w[:, :36].contiguous())      # K pitch not a multiple of 8 elements
+    # SwiGLU writes bf16 only and has no column scale
+    with pytest.raises(_lib.VllmB200Error, match="unsupported"):
+        o.linear(x, w, act="swiglu", out_dtype=torch.float32)
+    with pytest.raises(_lib.VllmB200Error, match="unsupported"):
+        o.linear(x, w, act="swiglu", colscale=torch.ones(64, dtype=torch.bfloat16, device="cuda"))
+    # output rows must start on 16-byte boundaries: ldc * element size % 16 != 0
+    for dt, ld in ((torch.bfloat16, 68), (torch.float32, 66)):
+        out = torch.empty(64, ld, dtype=dt, device="cuda")[:, :64]
+        with pytest.raises(_lib.VllmB200Error, match="misaligned"):
+            o.linear(x, w, out=out)
+    # the C ABI: a residual pitch below n_out is invalid; row_keep is refused with SwiGLU (by ops.linear too)
+    L = _lib.lib()
+    c = torch.empty(64, 64, dtype=torch.bfloat16, device="cuda")
+    res = torch.zeros(64, 64, dtype=torch.bfloat16, device="cuda")
+    keep = torch.ones(64, dtype=torch.uint8, device="cuda")
+    st = torch.cuda.current_stream().cuda_stream
+    args = (x.data_ptr(), 64, w.data_ptr(), 64, c.data_ptr(), 64, 64, 64, 64, None, None)
+    assert L.vllm_gemm_bf16(*args, res.data_ptr(), 56, 0, 0, st) == -1
+    assert L.vllm_gemm_bf16_rowmask(*args, None, 0, 4, 0, keep.data_ptr(), st) == -1
+    with pytest.raises(RuntimeError, match="not with swiglu"):
+        o.linear(x, w, act="swiglu", row_keep=keep.bool())
 
 
 @pytest.mark.parametrize("rows,cols", [(7, 3200), (1025, 3200), (300, 4096), (5, 256), (33, 12800)])

@@ -100,7 +100,7 @@ ATTN_DEFAULT, ATTN_WARP_MMA = 0, 1
 
 # the process-global path / tuning setters and the arguments that restore the library's own choice
 _KNOB_DEFAULTS = {"msda_set_variant": (MSDA_DEFAULT,), "msda_set_window": (0, 0, 0), "msda_set_window_fill": (-1,),
-                  "gemm_set_variant": (GEMM_DEFAULT,), "attention_set_variant": (ATTN_DEFAULT,)}
+                  "gemm_set_variant": (GEMM_DEFAULT,), "gemm_set_sm_limit": (0, 0), "attention_set_variant": (ATTN_DEFAULT,)}
 
 
 class VllmB200Error(RuntimeError):
