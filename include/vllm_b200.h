@@ -279,7 +279,8 @@ int vllm_rope_bf16(void* x, long long ld, const void* cos, const void* sin, long
  * bf16 views with explicit batch/token pitches in elements (heads contiguous, so a
  * packed qkv GEMM output is read in place); o: [batch, Tq, heads*head_dim] bf16.
  * kv_heads < heads = grouped-query attention.  seqlens (int32[batch], may be NULL):
- * keys >= seqlens[b] are masked (right padding / key_padding_mask); all query rows are computed.
+ * keys >= seqlens[b] are masked (right padding / key_padding_mask); a seqlens[b] >= Tk masks nothing and reads no
+ * key past Tk; all query rows are computed.
  * key_mask (uint8 [batch, Tk], may be NULL): 1 = attend, 0 = masked -- an arbitrary key_padding_mask
  * (nn.MultiheadAttention / GroundingDinoBiMultiHeadAttention semantics, inverted).
  * attn_mask (uint8 [batch*heads, Tq, Tk], may be NULL): 1 = attend; exactly the [N*H, L, S] tensor
@@ -289,9 +290,15 @@ int vllm_rope_bf16(void* x, long long ld, const void* cos, const void* sin, long
  * of an image; HF modeling_swin.py SwinSelfAttention.forward, used by the reference through AutoBackbone,
  * modeling_ov_grounding_dino_mask_dn.py:471-504).
  * causal != 0: query i sees keys <= i + (Tk - Tq).  head_dim in {32, 64, 128, 256}.
+ * scale must be > 0 and finite, else VLLM_EINVAL before anything runs (the wgmma kernel scales after the row max).
+ * A query row that can attend no key (seqlens 0, an all-0 key_mask or attn_mask row, a -inf bias row, causal rows
+ * i < Tq - Tk) is written as exact zeros.
+ * K / V rows that are masked (keys in [seqlens[b], Tk), key_mask 0) must still hold finite values on the default
+ * variant: the wgmma kernel multiplies them by P = 0, and NaN * 0 is NaN.  Rows past Tk are never read.
  * workspace (may be NULL): caller-owned scratch of workspace_bytes; when the query side alone cannot fill the
  * GPU (few queries, many keys: GDINO text->vision attention, 80 x 21760) the key axis is split across CTAs and
- * the partials (unnormalised O, running max, sum) are merged by a second kernel.  NULL only turns the split off. */
+ * the partials (unnormalised O, running max, sum) are merged by a second kernel.  NULL only turns the split off.
+ * n splits use the first batch*heads*n*Tq*(head_dim + 2) floats of it. */
 int vllm_attention_bf16(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk,
                         int heads, int kv_heads, int head_dim, long long q_batch_pitch,
                         long long q_token_pitch, long long k_batch_pitch, long long k_token_pitch,
@@ -323,6 +330,11 @@ int vllm_attention_bf16_tiles(const void* q, const void* k, const void* v, void*
 #define VLLM_ATTN_DEFAULT 0
 #define VLLM_ATTN_WARP_MMA 1
 int vllm_attention_set_variant(int variant);
+/* Split-KV count for tests (process-global): 0 (the default) lets the library choose; n in 1..64 makes every
+ * vllm_attention_bf16 call with a non-NULL workspace split the key axis n ways, on both the wgmma and the warp-MMA kernel
+ * and whatever the shape, masks or causal flag.  A NULL workspace, the window kernel and tile-list calls still do not
+ * split; a workspace smaller than n partials is VLLM_EINVAL.  Any other n: VLLM_EINVAL, nothing changes. */
+int vllm_attention_set_splits(int n);
 
 /* ---- tensor-parallel LLM decoder over peer memory (BASELINE cfg 5, SURVEY 8e) -------
  * The reference runs HF LlamaDecoderLayer unsharded (modeling_visionllmv2.py:724-732); the north-star splits it

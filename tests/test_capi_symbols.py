@@ -84,6 +84,13 @@ def test_round2_entry_points_marshal_and_accept_empty_problems():
     assert L.vllm_attention_mask_tiles(None, 4, 100, 100, None, None, None) < 0                                              # null pointers
     args = [None] * 4 + [0, 64, 64, 8, 8, 32] + [0] * 8 + [None, None, None, 1.0]
     assert L.vllm_attention_bf16_tiles(*args, None, None, None) < 0                                                          # no tile lists
+    assert L.vllm_attention_set_splits(64) == 0 and L.vllm_attention_set_splits(0) == 0
+    assert L.vllm_attention_set_splits(-1) < 0 and L.vllm_attention_set_splits(65) < 0                                      # not a split count
+    dense = lambda scale: L.vllm_attention_bf16(*args[:-1], None, 0, 0, scale, None, 0, None)                     # noqa: E731
+    tiles = lambda scale: L.vllm_attention_bf16_tiles(*args[:-2], 16, scale, 16, 16, None)   # never dereferenced  # noqa: E731
+    assert dense(0.125) == 0 and tiles(0.125) == 0
+    for bad in (0.0, -0.5, float("nan"), float("inf")):                                                                      # scale must be > 0, finite
+        assert dense(bad) < 0 and tiles(bad) < 0
     assert L.vllm_upsample_add_nhwc_bf16_ex(None, 10, None, None, 1, 8, 8, 16, 16, 256, 1, None) < 0                       # pitch < image
     assert L.vllm_sine_embed_f32(None, None, None, None, 1, 5, 0.0, None, 128, 0, None, 1024, 1, 0, 0, None, None) < 0    # > 4 features
     assert L.vllm_sine_embed_f32(None, None, None, None, 1, 2, 0.0, None, 100, 0, None, 256, 1, 0, 0, None, None) < 0     # nd % 8

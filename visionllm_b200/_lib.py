@@ -79,6 +79,7 @@ _SIGNATURES = {
                                        vp, vp, vp, cf, vp, vp, vp]),
     "vllm_attention_mask_tiles": (ci, [vp, cll, ci, ci, vp, vp, vp]),
     "vllm_attention_set_variant": (ci, [ci]),
+    "vllm_attention_set_splits": (ci, [ci]),
     "vllm_peer_alloc": (ci, [ctypes.POINTER(vp), ctypes.c_size_t]),
     "vllm_peer_free": (ci, [vp]),
     "vllm_peer_handle_bytes": (ci, []),
@@ -100,7 +101,8 @@ ATTN_DEFAULT, ATTN_WARP_MMA = 0, 1
 
 # the process-global path / tuning setters and the arguments that restore the library's own choice
 _KNOB_DEFAULTS = {"msda_set_variant": (MSDA_DEFAULT,), "msda_set_window": (0, 0, 0), "msda_set_window_fill": (-1,),
-                  "gemm_set_variant": (GEMM_DEFAULT,), "gemm_set_sm_limit": (0, 0), "attention_set_variant": (ATTN_DEFAULT,)}
+                  "gemm_set_variant": (GEMM_DEFAULT,), "gemm_set_sm_limit": (0, 0), "attention_set_variant": (ATTN_DEFAULT,),
+                  "attention_set_splits": (0,)}
 
 
 class VllmB200Error(RuntimeError):

@@ -82,7 +82,7 @@ flash_fwd_kernel(const AttnArgs a) {
   const int split = blockIdx.x % a.n_splits, mblk = blockIdx.x / a.n_splits, head = blockIdx.y, b = blockIdx.z;
   const int kvh = head / (a.heads / a.kv_heads);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int len = a.seqlens ? a.seqlens[b] : a.Tk;
+  const int len = a.seqlens ? min(a.seqlens[b], a.Tk) : a.Tk;
   const int m0 = mblk * BM;
 
   const __nv_bfloat16* qb = a.q + b * a.q_bs + (long long)head * D;
@@ -530,6 +530,17 @@ static int split_kv_count(const AttnArgs& a, int batch, int D, const SplitKv& f,
   return (int)best;
 }
 
+int g_attn_splits = 0;  // vllm_attention_set_splits: 0 = split_kv_count decides, 1..64 = that count
+
+// The split count of a call: the count forced by vllm_attention_set_splits, else split_kv_count's.  VLLM_EINVAL when the
+// workspace cannot hold the forced count's partials.  A NULL workspace and a tile-list call never split.
+static int splits_of(const AttnArgs& a, int batch, int D, const SplitKv& f, const void* workspace, long long workspace_bytes) {
+  if (!g_attn_splits) return split_kv_count(a, batch, D, f, workspace, workspace_bytes);
+  if (!workspace || a.tile_counts) return 1;
+  if ((long long)batch * a.heads * g_attn_splits * a.Tq * (D + 2) * 4 > workspace_bytes) return VLLM_EINVAL;
+  return g_attn_splits;
+}
+
 template <int D>
 static int launch_combine(const AttnArgs& a, int batch, cudaStream_t st) {
   const long long n_rows = (long long)batch * a.heads * a.Tq;
@@ -548,7 +559,8 @@ int launch(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long wo
   if (!per_sm && (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, flash_fwd_kernel<D, BN>, NW * 32, SMEM) != cudaSuccess ||
                   per_sm < 1))
     per_sm = 1;
-  a.n_splits = split_kv_count(a, batch, D, {BM, BN, per_sm, 8, 2, false}, workspace, workspace_bytes);
+  a.n_splits = splits_of(a, batch, D, {BM, BN, per_sm, 8, 2, false}, workspace, workspace_bytes);
+  if (a.n_splits < 1) return a.n_splits;
   a.ws = a.n_splits > 1 ? (float*)workspace : nullptr;
   dim3 grid((unsigned)(((a.Tq + BM - 1) / BM) * a.n_splits), a.heads, batch);
   flash_fwd_kernel<D, BN><<<grid, NW * 32, SMEM, st>>>(a);
@@ -558,10 +570,12 @@ int launch(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long wo
 
 // The wgmma kernel (attention_wgmma.cu) runs one CTA of 128 query rows per SM.  An unmasked head_dim-128 call never
 // splits, and only this family rejects empty splits: both as tuned so far (the split-KV re-tune, DESIGN §10 item 3).
+// A count forced by vllm_attention_set_splits overrides both.
 template <int D>
 static int launch_wgmma(AttnArgs a, int batch, cudaStream_t st, void* workspace, long long workspace_bytes) {
-  if (D == 128 && !a.key_mask) workspace = nullptr;
-  a.n_splits = split_kv_count(a, batch, D, {128, 64, 1, 4, 4, true}, workspace, workspace_bytes);
+  if (D == 128 && !a.key_mask && !g_attn_splits) workspace = nullptr;
+  a.n_splits = splits_of(a, batch, D, {128, 64, 1, 4, 4, true}, workspace, workspace_bytes);
+  if (a.n_splits < 1) return a.n_splits;
   a.ws = a.n_splits > 1 ? (float*)workspace : nullptr;
   const int rc = vllm_attention_wgmma(a, batch, D, st);
   return rc == VLLM_OK && a.n_splits > 1 ? launch_combine<D>(a, batch, st) : rc;
@@ -575,6 +589,11 @@ extern "C" int vllm_attention_set_variant(int v) {
   g_attn_variant = v;
   return VLLM_OK;
 }
+extern "C" int vllm_attention_set_splits(int n) {
+  if (n < 0 || n > 64) return VLLM_EINVAL;
+  g_attn_splits = n;
+  return VLLM_OK;
+}
 
 static int attention_impl(const void* q, const void* k, const void* v, void* o, int batch, int Tq, int Tk,
                           int heads, int kv_heads, int head_dim, long long q_batch_pitch,
@@ -585,6 +604,8 @@ static int attention_impl(const void* q, const void* k, const void* v, void* o, 
                           int causal, float scale, void* workspace, long long workspace_bytes, const int* tile_counts,
                           const int* tile_lists, void* stream) {
   if (batch < 0 || Tq < 0 || Tk < 0 || heads <= 0 || kv_heads <= 0 || heads % kv_heads) return VLLM_EINVAL;
+  // The wgmma kernel takes the row max of the unscaled scores: a scale <= 0 would turn the masked -inf into +inf / NaN.
+  if (!(scale > 0.f) || !isfinite(scale)) return VLLM_EINVAL;
   if ((tile_counts == nullptr) != (tile_lists == nullptr)) return VLLM_EINVAL;
   if (tile_counts && (!attn_mask || causal || (head_dim != 32 && head_dim != 64 && head_dim != 128))) return VLLM_EUNSUPPORTED;
   if (batch == 0 || Tq == 0) return VLLM_OK;

@@ -423,6 +423,9 @@ def attention(q, k, v, causal=False, scale=None, seqlens=None, key_mask=None, at
         raise RuntimeError("attention: inconsistent q/k/v shapes")
     if out is None:
         out = torch.empty((B, Tq, H * D), dtype=torch.bfloat16, device=q.device)
+    elif (out.dtype != torch.bfloat16 or out.device != q.device or tuple(out.shape) != (B, Tq, H * D)
+          or out.stride(2) != 1):
+        raise RuntimeError("attention: out must be a bf16 [B, Tq, H*D] tensor on q's device with contiguous rows")
     if scale is None:
         scale = D ** -0.5
     sl = None
