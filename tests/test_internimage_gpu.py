@@ -109,7 +109,11 @@ def test_dcnv3_prep_and_blend_match_torch(G, K, with_scale, pad):
         ref = core * (1 - s_) + xp * s_
     else:
         ref = core
-    assert out.dtype == torch.bfloat16 and torch.equal(out, ref.bfloat16()) or (out.float() - ref).abs().max() < 2e-2
+    assert out.dtype == torch.bfloat16
+    if with_scale:        # one bf16 rounding of the fp32 blend (tests/test_row_kernels_contract_gpu.py has the fp64 bound)
+        assert ((out.float() - ref).abs() <= 2.0 ** -8 * ref.abs()).all()
+    else:
+        assert torch.equal(out, ref.bfloat16())
 
 
 def test_layernorm_residual_matches_fp32():
