@@ -1,21 +1,37 @@
-"""GPU: TFLOP/s of the wgmma GEMM (both tile widths) at the hot-path shapes; torch.matmul (cuBLAS) beside it.
-Usage: python tools/gemm_bench.py [out.json]   (the card's name and power limit are recorded with the numbers)"""
-import json, os, subprocess, sys
+"""GPU: TFLOP/s of the wgmma GEMM (both tile widths, forced) at the hot-path shapes, each with the epilogue it runs in the model;
+torch.matmul (cuBLAS, no epilogue) beside it.  The three arms alternate, REPEATS rounds of each; the median and the spread
+(max - min over the rounds) are printed.  The card's name, power limit and clocks are read in the same call.
+Usage: python tools/gemm_bench.py [out.json] [shape ...]"""
+import json, os, statistics, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from visionllm_b200 import ops, _lib
 
-SHAPES = {"vit_qkv": (41000, 9600, 3200), "vit_proj": (41000, 3200, 3200), "vit_fc1": (41000, 12800, 3200),
-          "vit_fc2": (41000, 3200, 12800), "llm_qkv": (12288, 12288, 4096), "llm_gateup": (12288, 22016, 4096),
-          "llm_down": (12288, 4096, 11008), "gdino_ffn1": (21760 * 8, 2048, 256), "sq8k": (8192, 8192, 8192)}
-res = {"gpu": subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                             capture_output=True, text=True).stdout.strip()}
+# name: (M, N, K, epilogue); epilogue keys: bias, act, ls (column scale), res (residual), f32 (fp32 output)
+SHAPES = {
+    "vit_qkv": (41000, 9600, 3200, dict(bias=True)),
+    "vit_proj": (41000, 3200, 3200, dict(bias=True, ls=True, res=True)),
+    "vit_fc1": (41000, 12800, 3200, dict(bias=True, act="gelu")),
+    "vit_fc2": (41000, 3200, 12800, dict(bias=True, ls=True, res=True)),
+    "llm_qkv": (12288, 12288, 4096, dict()),
+    "llm_o": (12288, 4096, 4096, dict(res=True)),
+    "llm_gateup": (12288, 22016, 4096, dict(act="swiglu")),
+    "llm_down": (12288, 4096, 11008, dict(res=True)),
+    "lm_head": (12288, 32026, 4096, dict(f32=True)),
+    "gdino_ffn1": (21760 * 8, 2048, 256, dict(bias=True, act="relu")),
+    "sq8k": (8192, 8192, 8192, dict()),
+}
+REPEATS = 3
+ARMS = (("tile128x128", _lib.GEMM_NARROW_TILE), ("tile128x256", _lib.GEMM_WIDE_TILE), ("cublas", None))
 
 
-def timeit(fn, iters=10):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
+def gpu_state():
+    q = "name,power.limit,clocks.sm,clocks.max.sm,clocks_throttle_reasons.active"
+    return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True).stdout.strip()
+
+
+def timeit(fn, iters):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(iters):
@@ -24,23 +40,64 @@ def timeit(fn, iters=10):
     return e0.elapsed_time(e1) / iters
 
 
-for name, (M, N, K) in SHAPES.items():
-    x = torch.randn(M, K, device="cuda").bfloat16()
-    w = (torch.randn(N, K, device="cuda") / K ** 0.5).bfloat16()
-    out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
+def bench_shape(M, N, K, epi):
+    dev = "cuda"
+    x = torch.randn(M, K, device=dev).bfloat16()
+    w = (torch.randn(N, K, device=dev) / K ** 0.5).bfloat16()
+    act = epi.get("act")
+    n_out = N // 2 if act == "swiglu" else N
+    bias = torch.randn(N, device=dev).bfloat16() if epi.get("bias") else None
+    ls = torch.rand(N, device=dev).bfloat16() if epi.get("ls") else None
+    res = torch.randn(M, n_out, device=dev).bfloat16() if epi.get("res") else None
+    if epi.get("f32"):
+        out = torch.empty(M, (N + 7) // 8 * 8, device=dev, dtype=torch.float32)[:, :N]     # 16-byte row pitch, like the LLM logits
+    else:
+        out = torch.empty(M, n_out, device=dev, dtype=torch.bfloat16)
+    cb_out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+    ours = lambda: ops.linear(x, w, bias=bias, act=act, colscale=ls, residual=res, out=out)
+    cublas = lambda: torch.matmul(x, w.T, out=cb_out)
+    iters = max(3, min(20, int(2e13 / (2.0 * M * N * K))))       # about 40 ms of work per timing at ~500 TFLOP/s
+    times = {nm: [] for nm, _ in ARMS}
+    for nm, v in ARMS:                                           # warm every arm (module load, cuBLAS heuristics)
+        with _lib.knob("gemm_set_variant", v if v is not None else _lib.GEMM_DEFAULT):
+            (cublas if v is None else ours)()
+    torch.cuda.synchronize()
+    for _ in range(REPEATS):
+        for nm, v in ARMS:
+            if v is None:
+                times[nm].append(timeit(cublas, iters))
+            else:
+                with _lib.knob("gemm_set_variant", v):
+                    times[nm].append(timeit(ours, iters))
     fl = 2.0 * M * N * K
     r = {}
-    for v, nm in ((_lib.GEMM_DEFAULT, "tile128x128"), (_lib.GEMM_WIDE_TILE, "tile128x256")):
-        try:
-            with _lib.knob("gemm_set_variant", v):
-                ms = timeit(lambda: ops.linear(x, w, out=out))
-            r[f"{nm}_tflops"] = fl / ms / 1e9
-        except Exception as e:
-            r[f"{nm}_error"] = str(e)
-    ms = timeit(lambda: torch.matmul(x, w.T, out=out))
-    r["cublas_tflops"] = fl / ms / 1e9
-    res[name] = r
-    print(name, r, flush=True)
-    del x, w, out
-if len(sys.argv) > 1:
-    json.dump(res, open(sys.argv[1], "w"), indent=1)
+    for nm, ts in times.items():
+        tf = [fl / t / 1e9 for t in ts]
+        r[nm] = {"tflops_median": statistics.median(tf), "tflops_spread": max(tf) - min(tf), "ms_median": statistics.median(ts)}
+    return r
+
+
+def main():
+    args = sys.argv[1:]
+    out_path = args.pop(0) if args and args[0].endswith(".json") else None
+    names = args or list(SHAPES)
+    res = {"gpu_before": gpu_state()}
+    print("gpu (name, power limit, SM clock, max SM clock, throttle reasons):", res["gpu_before"], flush=True)
+    for name in names:
+        M, N, K, epi = SHAPES[name]
+        r = bench_shape(M, N, K, epi)
+        r["shape"] = [M, N, K]; r["epilogue"] = epi
+        res[name] = r
+        print(f"{name:11s} {M}x{N}x{K} {epi}: " +
+              "  ".join(f"{nm} {v['tflops_median']:.0f}±{v['tflops_spread']:.0f}" for nm, v in r.items() if isinstance(v, dict)
+                        and "tflops_median" in v), flush=True)
+        torch.cuda.empty_cache()
+    res["gpu_after"] = gpu_state()
+    print("gpu after:", res["gpu_after"], flush=True)
+    if out_path:
+        with open(out_path, "w") as f:
+            json.dump(res, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

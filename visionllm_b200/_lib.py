@@ -96,7 +96,7 @@ _SIGNATURES = {
 
 # values of vllm_msda_set_variant / vllm_gemm_set_variant / vllm_attention_set_variant (include/vllm_b200.h)
 MSDA_DEFAULT, MSDA_NO_HINT, MSDA_BF16_NO_WINDOW, MSDA_FP32_WINDOW = 0, 4, 32, 33
-GEMM_DEFAULT, GEMM_WIDE_TILE = 0, 2
+GEMM_DEFAULT, GEMM_WIDE_TILE, GEMM_NARROW_TILE = 0, 2, 3
 ATTN_DEFAULT, ATTN_WARP_MMA = 0, 1
 
 # the process-global path / tuning setters and the arguments that restore the library's own choice

@@ -14,14 +14,23 @@
 // Structure (persistent, warp-specialised, one CTA of three warpgroups per SM):
 //   warpgroup 0    producer: one elected lane of warp 0 issues the TMA loads, A tile 128x64 and B tile (256|128)x64
 //                  bf16, 128B swizzle, STAGES-deep mbarrier ring; the warpgroup hands its registers to the consumers
-//   warpgroups 1-2 consumers: warpgroup w owns rows 64(w-1)..64(w-1)+63 of the tile and issues wgmma m64n128k16
-//                  (one or two per k-step) straight from the swizzled stages; fp32 accumulators stay in registers
+//   warpgroups 1-2 consumers: warpgroup w owns rows 64(w-1)..64(w-1)+63 of the tile and issues one wgmma m64n{BN}k16
+//                  per k-step straight from the swizzled stages; fp32 accumulators stay in registers
 //                  (64 x BN / 128 threads = 64 | 128 per thread).  One k-block of MMAs stays in flight while the next
 //                  stage is awaited; a stage goes back to the producer when the MMAs that read it have retired.
 //                  The fused epilogue runs on the accumulator fragments (a thread owns column pairs of two rows, so
 //                  the SwiGLU (gate, up) pair never leaves a thread); bf16 output is staged per warp in shared memory
 //                  and leaves as 128-byte row runs; the producer keeps prefetching the next tile's stages meanwhile.
 // Tiles are visited in groups of GROUP_M row-blocks so concurrently running CTAs share B (weights) in L2.
+//
+// Instantiations gemm_bf16_wgmma_kernel<BN, TA, TB, EPI> (chosen per launch by pick_kernel, 17 in all):
+//   BN  128 | 256            tile width (vllm_gemm_set_variant; the scatter GEMM is always 256)
+//   TA, TB  0 | 1            K-major | MN-major operand: (0, 0) for every forward call, the other three for
+//                            vllm_gemm_bf16_tn / _batched (training)
+//   EPI  EPI_BF16 | EPI_GENERAL for every (BN, TA, TB); EPI_SCATTER only for <256, 0, 0>
+// The layout is a template parameter so that the k-block (fence, four MMAs, commit, wait) is one basic block: with a
+// run-time layout branch inside it, ptxas closes the wgmma group in each branch and the wait after the join retires
+// the k-block just issued.  tests/test_gemm_sass_cpu.py checks the SASS for it.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "vllm_b200.h"   // VLLM_GEMM_* variant names
@@ -84,7 +93,9 @@ __device__ __forceinline__ TilePlan plan_tile(const GemmArgs& g, int m0, int n0,
 template <int BN> struct Cfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BN == 256 ? 4 : 6;     // 192 KB of operand stages either way
+  // 192 KB of operand stages either way; a fifth 48 KB stage of the wide tile would need 240 KB, more than the 227 KB
+  // a block may use even without the epilogue staging
+  static constexpr int STAGES = BN == 256 ? 4 : 6;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2 * BN * 4 /*bias, scale*/ +
                               CONSUMER_WARPS * EPI_WARP_BYTES /*per-warp store staging*/;
 };
@@ -102,28 +113,38 @@ __device__ __forceinline__ void tile_coords(int t, int tiles_m, int tiles_n, int
   tn = in / gsz;
 }
 
-// the four operand-layout combinations of one k-block (BK = 4 k-steps) of a warpgroup's 64 x BN tile
-template <int TA, int TB, int NB>
-__device__ __forceinline__ void mma_kblock(float (&acc)[NB][64], uint32_t sa, uint32_t sb, bool first_kb) {
+// one k-block (BK = 4 k-steps) of a warpgroup's 64 x BN tile: one m64n{BN}k16 per k-step.  B descriptor: K-major, BN
+// rows of 128 B in 8-row groups 1 KB apart (SBO); MN-major, BN / 64 chunks of 64 columns 8 KB apart (LBO).
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, uint32_t sb, bool first_kb) {
   // K-major: a k-step of 16 bf16 advances the start address by 32 B inside the 128 B swizzle row;
   // MN-major: by 16 k-rows x 128 B = 2 KB (descriptor address units are 16 B)
   const uint64_t adesc = TA ? tc::wgmma_desc_sw128(sa, 8192, 1024) : tc::wgmma_desc_sw128(sa, 16, 1024);
   const uint64_t bdesc = TB ? tc::wgmma_desc_sw128(sb, 8192, 1024) : tc::wgmma_desc_sw128(sb, 16, 1024);
   constexpr uint64_t astep = TA ? 128 : 2, bstep = TB ? 128 : 2;
-  constexpr uint64_t bhalf = 16384 >> 4;     // columns 128.. of the B tile: 128 K-major rows or two MN-major chunks
 #pragma unroll
-  for (int k = 0; k < BK / 16; ++k)
-#pragma unroll
-    for (int nb = 0; nb < NB; ++nb)
-      tc::wgmma_m64n128k16_ss<TA, TB>(acc[nb], adesc + astep * k, bdesc + bstep * k + bhalf * nb, !(first_kb && k == 0));
+  for (int k = 0; k < BK / 16; ++k) {
+    if constexpr (BN == 256)
+      tc::wgmma_m64n256k16_ss<TA, TB>(acc, adesc + astep * k, bdesc + bstep * k, !(first_kb && k == 0));
+    else
+      tc::wgmma_m64n128k16_ss<TA, TB>(acc, adesc + astep * k, bdesc + bstep * k, !(first_kb && k == 0));
+  }
 }
 
-template <int BN>
+// Epilogue of a launch (a template parameter: each instantiation carries only its own store path)
+//   EPI_BF16     bf16 output, no SwiGLU, N % 64 == 0: every 64-column chunk is staged per warp and leaves as 128-byte rows
+//   EPI_GENERAL  fp32 output, SwiGLU or ragged N: each fragment pair goes straight to global memory
+//   EPI_SCATTER  EPI_BF16 into the peer slots of vllm_gemm_bf16_scatter, then one flag arrival per consumer warp and tile
+enum { EPI_BF16 = 0, EPI_GENERAL = 1, EPI_SCATTER = 2 };
+
+// TA / TB = 1: that operand is MN-major (vllm_gemm_bf16_tn / _batched); the layout is fixed per instantiation so that
+// the k-block body is one basic block and one wgmma group stays in flight across k-blocks.
+template <int BN, int TA, int TB, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                        const GemmArgs g) {
   using C_ = Cfg<BN>;
-  constexpr int STAGES = C_::STAGES, NB = BN / 128;
+  constexpr int STAGES = C_::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - tc::smem_u32(smem_raw));
@@ -159,9 +180,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         if (tp.skip) continue;
         const int bt_m0 = g.bt_rows ? (tm * BM) / g.bt_rows * g.bt_rows : 0;
         // K-major A: global stacked row; MN-major A: column inside its matrix (the stack runs along the K rows)
-        const int row_a = tm * BM - (g.a_mn ? bt_m0 : 0);
-        const int row_b = tn * BN + (g.b_mn ? 0 : tp.b_row_off);
-        const int ka_off = g.a_mn ? tp.k_off : 0, kb_off = g.b_mn ? tp.k_off : 0;
+        const int row_a = tm * BM - (TA ? bt_m0 : 0);
+        const int row_b = tn * BN + (TB ? 0 : tp.b_row_off);
+        const int ka_off = TA ? tp.k_off : 0, kb_off = TB ? tp.k_off : 0;
         for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
           tc::mbar_wait(empty_bar(stage), phase ^ 1);
           const uint32_t sa = smem_base + stage * C_::STAGE_BYTES, sb = sa + A_BYTES;
@@ -172,12 +193,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             ra = row_a + seg * g.a_seg_rows;
           }
           tc::mbar_arrive_expect_tx(full_bar(stage), C_::STAGE_BYTES);
-          if (g.a_mn) {
+          if constexpr (TA) {
             for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
           } else {
             tc::tma_load_2d(sa, &tmap_a, full_bar(stage), ka, ra);
           }
-          if (g.b_mn) {
+          if constexpr (TB) {
             for (int h = 0; h < BN / 64; ++h)
               tc::tma_load_2d(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
           } else {
@@ -195,9 +216,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   const int wg = (warp - 4) >> 2;                  // 0 / 1: rows 0-63 / 64-127 of the tile
   const int et = threadIdx.x - 128;                // 0..255
   const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
-  const bool swiglu = g.act == ACT_SWIGLU;
+  const bool swiglu = EPI == EPI_GENERAL && g.act == ACT_SWIGLU;
   int stage = 0; uint32_t phase = 0;
-  float acc[NB][64];
+  float acc[BN / 2];
   for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     int tm, tn; tile_coords(t, g.tiles_m, g.tiles_n, g.group_m, tm, tn);
     const TilePlan tp = plan_tile(g, tm * BM, tn * BN, BM, num_kb);
@@ -215,14 +236,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       tc::mbar_wait(full_bar(stage), phase);
       const uint32_t sa = smem_base + stage * C_::STAGE_BYTES + wg * 8192, sb = smem_base + stage * C_::STAGE_BYTES + A_BYTES;
       const bool first = kb == tp.kb0;
-#pragma unroll
-      for (int nb = 0; nb < NB; ++nb) tc::acc_fence(acc[nb]);
+      tc::acc_fence(acc);
       tc::wgmma_fence();
-      if (g.a_mn) {
-        if (g.b_mn) mma_kblock<1, 1, NB>(acc, sa, sb, first); else mma_kblock<1, 0, NB>(acc, sa, sb, first);
-      } else {
-        if (g.b_mn) mma_kblock<0, 1, NB>(acc, sa, sb, first); else mma_kblock<0, 0, NB>(acc, sa, sb, first);
-      }
+      mma_kblock<BN, TA, TB>(acc, sa, sb, first);
       tc::wgmma_commit();
       tc::wgmma_wait<1>();                           // the previous k-block's MMAs have retired: its stage is free
       if (prev_stage >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev_stage));
@@ -230,8 +246,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
     tc::wgmma_wait<0>();
-#pragma unroll
-    for (int nb = 0; nb < NB; ++nb) tc::acc_fence(acc[nb]);
+    tc::acc_fence(acc);
     if (lane == 0) tc::mbar_arrive(empty_bar(prev_stage));
     tc::named_bar_sync(1, CONSUMER_THREADS);         // s_bias / s_scale of this tile are in place
 
@@ -259,7 +274,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     };
     // destination of an output row: C, or the peer slot that owns row block d of C (scatter mode)
     auto out_row = [&](int row) -> __nv_bfloat16* {
-      if (!g.sc_rows) return reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc;
+      if constexpr (EPI != EPI_SCATTER) return reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc;
       const int d = row / g.sc_rows;
       return reinterpret_cast<__nv_bfloat16*>(g.sc_dst[d]) + (size_t)(row - d * g.sc_rows) * g.ldc;
     };
@@ -287,27 +302,25 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     const int row0 = tm * BM + frag_row;
     const int warp_row0 = tm * BM + wg * 64 + (warp & 3) * 16;
     uint8_t* my_stage = s_epi + (warp - 4) * EPI_WARP_BYTES;
+    // n8 block j (columns 8j..8j+7 of the tile) is acc[4j..4j+3]
 #pragma unroll
-    for (int nb = 0; nb < NB; ++nb) {
+    for (int ch = 0; ch < BN / 64; ++ch) {           // 64-column chunks of the tile
+      const int c0 = ch * 64;
+      if (n0 + c0 >= g.N) break;                     // uniform
+      if constexpr (EPI == EPI_GENERAL) {
 #pragma unroll
-      for (int ch = 0; ch < 2; ++ch) {               // 64-column chunks of this 128-column accumulator half
-        const int c0 = nb * 128 + ch * 64;
-        if (n0 + c0 >= g.N) break;                   // uniform
-        if (swiglu || g.out_f32 || n0 + c0 + 64 > g.N) {
-#pragma unroll
-          for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
-            const int c = nb * 128 + 8 * j + frag_col;
-            emit(row0, c, acc[nb][4 * j], acc[nb][4 * j + 1]);
-            emit(row0 + 8, c, acc[nb][4 * j + 2], acc[nb][4 * j + 3]);
-          }
-          continue;
+        for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
+          const int c = 8 * j + frag_col;
+          emit(row0, c, acc[4 * j], acc[4 * j + 1]);
+          emit(row0 + 8, c, acc[4 * j + 2], acc[4 * j + 3]);
         }
-        // bf16 fast path: the warp stages its 16 rows x 64 columns in shared memory, then stores 128-byte row runs
+      } else {
+        // bf16: the warp stages its 16 rows x 64 columns in shared memory, then stores 128-byte row runs
         // (4-byte stores from the fragments would cost the L2 eight requests per 128-byte line instead of one)
 #pragma unroll
         for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
-          const int c = nb * 128 + 8 * j + frag_col;
-          float a0 = acc[nb][4 * j], a1 = acc[nb][4 * j + 1], b0 = acc[nb][4 * j + 2], b1 = acc[nb][4 * j + 3];
+          const int c = 8 * j + frag_col;
+          float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
           math(row0, c, a0, a1);
           math(row0 + 8, c, b0, b1);
           const int off = (8 * (j - 8 * ch) + frag_col) * 2;
@@ -324,7 +337,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         __syncwarp();
       }
     }
-    if (g.sc_rows) {                                 // tile pushed: publish it to the owner of these rows
+    if constexpr (EPI == EPI_SCATTER) {                                 // tile pushed: publish it to the owner of these rows
       __threadfence_system();
       __syncwarp();
       if (lane == 0 && warp_row0 < g.M)
@@ -340,10 +353,27 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 // whose epilogue stores ride NVLink while the other micro-batch's GEMM runs beside it (visionllm_b200/tp.py).
 int g_sm_limit = 0, g_scatter_sm_limit = 0;
 
-// VLLM_GEMM_DEFAULT: 128 x 128 tiles (faster than 128 x 256 at every hot-path shape measured on an H100, README.md);
-// VLLM_GEMM_WIDE_TILE forces the 256-column tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its
-// receivers count arrivals per such tile.
+// VLLM_GEMM_DEFAULT: the tile width of wide_by_shape(); VLLM_GEMM_WIDE_TILE / _NARROW_TILE force the 256- / 128-column
+// tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its receivers count arrivals per such tile.
 int g_gemm_variant = VLLM_GEMM_DEFAULT;
+
+using KernelFn = void (*)(const CUtensorMap, const CUtensorMap, const GemmArgs);
+
+// The instantiation of a launch: operand layouts from g.a_mn / g.b_mn, epilogue from the store kind (see EPI_*).
+template <int BN, int TA, int TB>
+KernelFn pick_epilogue(const GemmArgs& g) {
+  if (g.sc_rows) {
+    if constexpr (BN == 256 && !TA && !TB) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_SCATTER>;
+    return nullptr;
+  }
+  if (g.act == ACT_SWIGLU || g.out_f32 || g.N % 64) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_GENERAL>;
+  return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_BF16>;
+}
+template <int BN>
+KernelFn pick_kernel(const GemmArgs& g) {
+  if (g.a_mn) return g.b_mn ? pick_epilogue<BN, 1, 1>(g) : pick_epilogue<BN, 1, 0>(g);
+  return g.b_mn ? pick_epilogue<BN, 0, 1>(g) : pick_epilogue<BN, 0, 0>(g);
+}
 
 template <int BN>
 int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cudaStream_t st, long long a_rows = -1,
@@ -369,17 +399,33 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
   // Rasterisation: a group of `group_m` row-blocks sweeps all column-blocks before the next group starts, so one wave of
   // CTAs covers a near-square patch of tiles (minimal A+B bytes per wave).
   g.group_m = 8;
-  const cudaError_t e = vllm_smem_optin(gemm_bf16_wgmma_kernel<BN>, C_::SMEM);
+  const KernelFn kern = pick_kernel<BN>(g);
+  if (!kern) return VLLM_EUNSUPPORTED;
+  const cudaError_t e = vllm_smem_optin(kern, C_::SMEM);
   if (e != cudaSuccess) return (int)e;
-  gemm_bf16_wgmma_kernel<BN><<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, g);
+  kern<<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, g);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
+}
+
+// Default tile width of a dense K-major GEMM: 128 x 256 when the output is narrow (N <= 4096) and K is long (>= 3072),
+// else 128 x 128.  tools/gemm_bench.py, TFLOP/s 128 x 128 / 128 x 256, each shape with its model epilogue (H100 80GB
+// HBM3, 700 W power limit, median of 3):
+//   wide:   ViT proj 41000x3200x3200 370 / 409, fc2 41000x3200x12800 443 / 572, LLM down 12288x4096x11008 472 / 543,
+//           LLM o 12288x4096x4096 424 / 409 (a tie within the spread)
+//   narrow: ViT qkv 41000x9600x3200 594 / 430, fc1 (GELU) 41000x12800x3200 533 / 259, LLM qkv 12288^2x4096 558 / 439,
+//           gate|up (SwiGLU) 12288x22016x4096 537 / 420, lm_head (fp32) 12288x32026x4096 582 / 312,
+//           GDINO FFN 174080x2048x256 133 / 63, 8192^3 611 / 517
+// MN-major, batched and implicit-convolution launches were not measured at the wide tile and keep 128 x 128.
+bool wide_by_shape(const GemmArgs& g) {
+  return !g.a_mn && !g.b_mn && !g.bt_rows && !g.a_seg_kb && g.N <= 4096 && g.K >= 3072;
 }
 
 int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmArgs& g, cudaStream_t st, long long a_rows = -1,
                      int a_cols = -1) {
   // the receivers of a scatter GEMM count 8 arrivals per 128 x 256 tile (visionllm_b200/tp.py)
-  const bool wide = g.sc_rows || g_gemm_variant == VLLM_GEMM_WIDE_TILE;
+  const bool wide = g.sc_rows || g_gemm_variant == VLLM_GEMM_WIDE_TILE ||
+                    (g_gemm_variant == VLLM_GEMM_DEFAULT && wide_by_shape(g));
   return wide ? launch_gemm<256>(A, lda, B, ldb, g, st, a_rows, a_cols) : launch_gemm<128>(A, lda, B, ldb, g, st, a_rows, a_cols);
 }
 
@@ -388,7 +434,7 @@ int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmA
 extern "C" {
 
 int vllm_gemm_set_variant(int v) {
-  if (v != VLLM_GEMM_DEFAULT && v != VLLM_GEMM_WIDE_TILE) return VLLM_EINVAL;
+  if (v != VLLM_GEMM_DEFAULT && v != VLLM_GEMM_WIDE_TILE && v != VLLM_GEMM_NARROW_TILE) return VLLM_EINVAL;
   g_gemm_variant = v;
   return VLLM_OK;
 }
