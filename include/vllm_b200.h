@@ -195,7 +195,7 @@ int vllm_conv_rows_bf16(const void* xpad, long long pad_pixels, int channels, in
                         int kernel_w, const void* weight, int ldw, void* out, int ldo, int out_channels,
                         const void* bias, int act, void* stream);
 /* Tile selection for tests and sweeps (process-global): VLLM_GEMM_DEFAULT = the library's choice per launch (128 x 256
- * tiles for dense K-major GEMMs with N <= 4096 and K >= 3072, else 128 x 128; csrc/gemm.cu), VLLM_GEMM_WIDE_TILE =
+ * tiles for dense K-major GEMMs with N >= 2048, else 128 x 128; csrc/gemm.cu), VLLM_GEMM_WIDE_TILE =
  * 128 x 256 tiles, which the scatter GEMM always uses, VLLM_GEMM_NARROW_TILE = 128 x 128 tiles except for the scatter
  * GEMM.  Any other value: VLLM_EINVAL, nothing changes. */
 #define VLLM_GEMM_DEFAULT 0

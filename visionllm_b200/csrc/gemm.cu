@@ -19,15 +19,18 @@
 //                  (64 x BN / 128 threads = 64 | 128 per thread).  One k-block of MMAs stays in flight while the next
 //                  stage is awaited; a stage goes back to the producer when the MMAs that read it have retired.
 //                  The fused epilogue runs on the accumulator fragments (a thread owns column pairs of two rows, so
-//                  the SwiGLU (gate, up) pair never leaves a thread); bf16 output is staged per warp in shared memory
-//                  and leaves as 128-byte row runs; the producer keeps prefetching the next tile's stages meanwhile.
+//                  the SwiGLU (gate, up) pair never leaves a thread).  Its operands never stall a consumer: bias,
+//                  column scale and row mask of a tile come in by cp.async when the tile starts, and the first two
+//                  16 x 128 B residual chunks of each warp by TMA, all under the main loop.  Each consumer warp owns
+//                  two 16-row x 128-byte staging buffers (128B swizzle): the result of a chunk is written in place
+//                  over its residual and leaves by one TMA store; the producer keeps prefetching the next tile meanwhile.
 // Tiles are visited in groups of GROUP_M row-blocks so concurrently running CTAs share B (weights) in L2.
 //
-// Instantiations gemm_bf16_wgmma_kernel<BN, TA, TB, EPI> (chosen per launch by pick_kernel, 17 in all):
+// Instantiations gemm_bf16_wgmma_kernel<BN, TA, TB, EPI> (chosen per launch by pick_kernel, 19 in all):
 //   BN  128 | 256            tile width (vllm_gemm_set_variant; the scatter GEMM is always 256)
 //   TA, TB  0 | 1            K-major | MN-major operand: (0, 0) for every forward call, the other three for
 //                            vllm_gemm_bf16_tn / _batched (training)
-//   EPI  EPI_BF16 | EPI_GENERAL for every (BN, TA, TB); EPI_SCATTER only for <256, 0, 0>
+//   EPI  EPI_BF16 | EPI_F32 for every (BN, TA, TB); EPI_SWIGLU for <BN, 0, 0>; EPI_SCATTER only for <256, 0, 0>
 // The layout is a template parameter so that the k-block (fence, four MMAs, commit, wait) is one basic block: with a
 // run-time layout branch inside it, ptxas closes the wgmma group in each branch and the wait after the join retires
 // the k-block just issued.  tests/test_gemm_sass_cpu.py checks the SASS for it.
@@ -39,8 +42,8 @@ namespace {
 
 constexpr int BM = 128, BK = 64, THREADS = 384, CONSUMER_WARPS = 8, CONSUMER_THREADS = CONSUMER_WARPS * 32;
 constexpr int A_BYTES = BM * BK * 2;
-constexpr int EPI_PITCH = 128 + 16;                 // 64 bf16 columns + 16 B pad: conflict-free fragment writes and 16-byte reads
-constexpr int EPI_WARP_BYTES = 16 * EPI_PITCH;      // a consumer warp's 16 rows of one 64-column chunk
+constexpr int EPI_BUF = 16 * 128;                   // a staging buffer: a consumer warp's 16 rows x 128 B, 128B swizzle
+constexpr int SMEM_LIMIT = 232448;                  // 227 KB: the most shared memory an sm_90 block may opt in to
 
 enum { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3, ACT_SWIGLU = 4, ACT_QUICKGELU = 5 };
 
@@ -96,8 +99,17 @@ template <int BN> struct Cfg {
   // 192 KB of operand stages either way; a fifth 48 KB stage of the wide tile would need 240 KB, more than the 227 KB
   // a block may use even without the epilogue staging
   static constexpr int STAGES = BN == 256 ? 4 : 6;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + 2 * BN * 4 /*bias, scale*/ +
-                              CONSUMER_WARPS * EPI_WARP_BYTES /*per-warp store staging*/;
+  // after the stages (1024-aligned, as the 128B swizzle of the staging buffers requires): two staging buffers per
+  // consumer warp, the mbarriers, then the tile's bias and column scale (bf16, BN columns + one word for a start that
+  // is only 2-byte aligned) and row mask (BM bytes + one word), as cp_async_vec_word lays them out
+  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFF = EPI_OFF + CONSUMER_WARPS * 2 * EPI_BUF;
+  static constexpr int BIAS_OFF = BAR_OFF + 256;
+  static constexpr int SCALE_OFF = BIAS_OFF + 2 * BN + 4;
+  static constexpr int KEEP_OFF = SCALE_OFF + 2 * BN + 4;
+  static constexpr int SMEM = 1024 /*align*/ + KEEP_OFF + BM + 4;
+  static_assert(8 * (2 * STAGES + 2 * CONSUMER_WARPS) <= 256, "mbarriers overflow their slot");
+  static_assert(SMEM <= SMEM_LIMIT, "shared memory over the per-block limit");
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
@@ -131,29 +143,39 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint32_t sa, ui
   }
 }
 
-// Epilogue of a launch (a template parameter: each instantiation carries only its own store path)
-//   EPI_BF16     bf16 output, no SwiGLU, N % 64 == 0: every 64-column chunk is staged per warp and leaves as 128-byte rows
-//   EPI_GENERAL  fp32 output, SwiGLU or ragged N: each fragment pair goes straight to global memory
-//   EPI_SCATTER  EPI_BF16 into the peer slots of vllm_gemm_bf16_scatter, then one flag arrival per consumer warp and tile
-enum { EPI_BF16 = 0, EPI_GENERAL = 1, EPI_SCATTER = 2 };
+// Epilogue of a launch (a template parameter: each instantiation carries only its own store path).  Every kind works in
+// units: a unit is 16 rows x 128 B of output per consumer warp, staged in one of the warp's two buffers and stored by TMA
+// (the tensor map clips the M and N tails).
+//   EPI_BF16     bf16 output: a unit is 64 columns of the tile
+//   EPI_SWIGLU   bf16 output of SwiGLU: a unit is 128 columns of the tile, (gate, up) pairs -> 64 output columns
+//   EPI_F32      fp32 output: a unit is 64 columns of the tile, 256 B per row, so it takes both buffers
+//   EPI_SCATTER  EPI_BF16 (no bias, scale, residual or mask) into the peer slots of vllm_gemm_bf16_scatter by 16-byte
+//                stores from the staging buffer, then one flag arrival per consumer warp and tile
+// A residual unit (64 bf16 columns, 128 B per row) is TMA-loaded into the unit's buffer (EPI_F32: buffer 0) and completes
+// on that buffer's mbarrier; the thread that owns a fragment pair reads its residual and writes its result in place.
+enum { EPI_BF16 = 0, EPI_SWIGLU = 1, EPI_F32 = 2, EPI_SCATTER = 3 };
+
+// byte offset of (row r, byte b) in a 16-row x 128-byte buffer with the 128B swizzle of TMA (16-byte chunk b / 16 of
+// row r sits at chunk (b / 16) ^ (r % 8); the buffer is 1024-byte aligned): the eight rows a fragment instruction touches
+// (lane / 4) land in eight different bank groups
+__device__ __forceinline__ int swz(int r, int b) { return r * 128 + ((((b >> 4) ^ r) & 7) << 4) + (b & 15); }
 
 // TA / TB = 1: that operand is MN-major (vllm_gemm_bf16_tn / _batched); the layout is fixed per instantiation so that
 // the k-block body is one basic block and one wgmma group stays in flight across k-blocks.
 template <int BN, int TA, int TB, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_c, const __grid_constant__ CUtensorMap tmap_r,
                        const GemmArgs g) {
   using C_ = Cfg<BN>;
   constexpr int STAGES = C_::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - tc::smem_u32(smem_raw));
-  const uint32_t bar_base = smem_base + STAGES * C_::STAGE_BYTES;
+  const uint32_t bar_base = smem_base + C_::BAR_OFF;
   auto full_bar = [&](int s) { return bar_base + 8 * s; };
   auto empty_bar = [&](int s) { return bar_base + 8 * (STAGES + s); };
-  float* s_bias = reinterpret_cast<float*>(smem_gen + STAGES * C_::STAGE_BYTES + 256);
-  float* s_scale = s_bias + BN;
-  uint8_t* s_epi = reinterpret_cast<uint8_t*>(s_scale + BN);   // CONSUMER_WARPS x 16 rows x EPI_PITCH bytes
+  auto res_bar = [&](int i) { return bar_base + 8 * (2 * STAGES + i); };   // buffer i of the staging (2 per consumer warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = g.tiles_m * g.tiles_n;
@@ -162,9 +184,14 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if (warp == 0 && lane == 0) {
     tc::tma_prefetch_desc(&tmap_a);
     tc::tma_prefetch_desc(&tmap_b);
+    if constexpr (EPI != EPI_SCATTER) {
+      tc::tma_prefetch_desc(&tmap_c);
+      if (g.residual) tc::tma_prefetch_desc(&tmap_r);
+    }
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) { tc::mbar_init(full_bar(s), 1); tc::mbar_init(empty_bar(s), CONSUMER_WARPS); }
+    for (int i = 0; i < 2 * CONSUMER_WARPS; ++i) tc::mbar_init(res_bar(i), 1);
     tc::mbar_fence_init();
   }
   __syncthreads();
@@ -214,9 +241,29 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   // ===================== consumers: main loop + epilogue =====================
   tc::reg_alloc<232>();
   const int wg = (warp - 4) >> 2;                  // 0 / 1: rows 0-63 / 64-127 of the tile
+  const int cw = warp - 4;                         // consumer warp 0..7: rows 16 cw .. 16 cw + 15 of the tile
   const int et = threadIdx.x - 128;                // 0..255
-  const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
-  const bool swiglu = EPI == EPI_GENERAL && g.act == ACT_SWIGLU;
+  const int lr = lane >> 2, frag_col = 2 * (lane & 3);   // fragment rows lr, lr + 8 of the warp; column pair base
+  const bool has_res = EPI != EPI_SCATTER && g.residual != nullptr;
+  constexpr int UNIT_COLS = EPI == EPI_SWIGLU ? 128 : 64;   // tile columns per unit
+  constexpr int UNITS = BN / UNIT_COLS;
+  constexpr int RES_AHEAD = EPI == EPI_F32 ? 1 : 2;         // residual units in flight (EPI_F32 stores from both buffers)
+  const int n_out = EPI == EPI_SWIGLU ? g.N / 2 : g.N;
+  uint8_t* s_buf = smem_gen + C_::EPI_OFF + cw * 2 * EPI_BUF;
+  const uint32_t s_buf_u32 = smem_base + C_::EPI_OFF + cw * 2 * EPI_BUF;
+  const uint32_t s_bias = smem_base + C_::BIAS_OFF, s_scale = smem_base + C_::SCALE_OFF, s_keep = smem_base + C_::KEEP_OFF;
+  // column 0 / row 0 of a tile in those vectors: the tile starts at a multiple of 256 / 128 bytes of the global vector,
+  // so its offset inside the first word is that of the vector's base
+  const __nv_bfloat16* bias_t = reinterpret_cast<const __nv_bfloat16*>(smem_gen + C_::BIAS_OFF + (reinterpret_cast<uintptr_t>(g.bias) & 3));
+  const __nv_bfloat16* scale_t =
+      reinterpret_cast<const __nv_bfloat16*>(smem_gen + C_::SCALE_OFF + (reinterpret_cast<uintptr_t>(g.colscale) & 3));
+  const uint8_t* keep_t = smem_gen + C_::KEEP_OFF + (reinterpret_cast<uintptr_t>(g.row_keep) & 3);
+  // a missing bias / column scale reads as 0 / 1 for every tile: the arithmetic stays that of a present one
+  if (et <= BN / 2) {
+    if (!g.bias) *reinterpret_cast<uint32_t*>(smem_gen + C_::BIAS_OFF + 4 * et) = 0u;
+    if (!g.colscale) *reinterpret_cast<uint32_t*>(smem_gen + C_::SCALE_OFF + 4 * et) = 0x3F803F80u;   // bf16 1.0, 1.0
+  }
+  uint32_t res_phase = 0;                          // bit b: parity of the next completion of buffer b's mbarrier
   int stage = 0; uint32_t phase = 0;
   float acc[BN / 2];
   for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
@@ -224,12 +271,24 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     const TilePlan tp = plan_tile(g, tm * BM, tn * BN, BM, num_kb);
     if (tp.skip) continue;
     const int n0 = tn * BN;
-    // bias / column scale of the tile go to shared memory now (broadcast reads in the epilogue math), so their global-load
-    // latency hides under the main loop; the previous tile's readers left at the barrier that closed its epilogue
-    if (et < BN) {
-      const int col = n0 + et;
-      s_bias[et] = (g.bias && col < g.N) ? __bfloat162float(g.bias[col]) : 0.f;
-      s_scale[et] = (g.colscale && col < g.N) ? __bfloat162float(g.colscale[col]) : 1.f;
+    const int oc0 = EPI == EPI_SWIGLU ? n0 / 2 : n0;            // the tile's first output column
+    const int warp_row0 = tm * BM + cw * 16;
+    const bool warp_live = warp_row0 < g.M;                     // uniform: the warp has rows to store
+    // Operands of the epilogue, requested now so they arrive under the main loop.  The previous tile's readers of
+    // s_bias / s_scale / s_keep left at the barrier that closed its epilogue.
+    if (g.bias && et <= BN / 2) tc::cp_async_vec_word(s_bias, g.bias, 2LL * g.N, 2LL * n0, et);
+    if (g.colscale && et <= BN / 2) tc::cp_async_vec_word(s_scale, g.colscale, 2LL * g.N, 2LL * n0, et);
+    if (g.row_keep && et <= BM / 4) tc::cp_async_vec_word(s_keep, g.row_keep, g.M, (long long)tm * BM, et);
+    auto load_res = [&](int u) {                               // lane 0: residual unit u into its buffer
+      const int b = EPI == EPI_F32 ? 0 : (u & 1);
+      tc::mbar_arrive_expect_tx(res_bar(2 * cw + b), EPI_BUF);
+      tc::tma_load_2d(s_buf_u32 + b * EPI_BUF, &tmap_r, res_bar(2 * cw + b), oc0 + 64 * u, warp_row0);
+    };
+    if (has_res && warp_live && lane == 0) {
+      tc::bulk_wait_read<0>();                     // the previous tile's stores have read both buffers
+#pragma unroll
+      for (int u = 0; u < RES_AHEAD && u < UNITS; ++u)
+        if (oc0 + 64 * u < n_out) load_res(u);
     }
     int prev_stage = -1;
     for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
@@ -248,103 +307,172 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     tc::wgmma_wait<0>();
     tc::acc_fence(acc);
     if (lane == 0) tc::mbar_arrive(empty_bar(prev_stage));
-    tc::named_bar_sync(1, CONSUMER_THREADS);         // s_bias / s_scale of this tile are in place
+    tc::cp_async_wait_all();
+    tc::named_bar_sync(1, CONSUMER_THREADS);         // every thread's cp.async of s_bias / s_scale / s_keep has landed
 
-    // ---- epilogue on the accumulator fragments: element pair (c, c + 1) of rows r and r + 8 per n8 block ----
-    // bias -> activation -> column scale -> residual -> row mask on the pair (c, c + 1) of `row` (not for SwiGLU)
-    auto math = [&](int row, int c, float& v0, float& v1) {
-      const int col = n0 + c;
-      v0 += s_bias[c]; v1 += s_bias[c + 1];
-      if (g.act == ACT_GELU) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
-      else if (g.act == ACT_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-      else if (g.act == ACT_SILU) { v0 = silu(v0); v1 = silu(v1); }
-      else if (g.act == ACT_QUICKGELU) { v0 = v0 / (1.f + __expf(-1.702f * v0)); v1 = v1 / (1.f + __expf(-1.702f * v1)); }
-      v0 *= s_scale[c]; v1 *= s_scale[c + 1];
-      if (row >= g.M) return;
-      if (g.residual) {
-        const __nv_bfloat16* rp = g.residual + (size_t)row * g.ldr + col;
-        if (col + 1 < g.N) {                         // col is even: a pair is 4-byte aligned
-          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rp));
-          v0 += f.x; v1 += f.y;
+    // ---- epilogue on the accumulator fragments: n8 block j (columns 8j..8j+7 of the tile) is acc[4j..4j+3], the pair
+    // (c, c + 1) of rows lr and lr + 8 of the warp.  Order per element: +bias -> act -> *scale -> +residual -> row mask,
+    // each an fp32 operation of its own (no contraction), then one rounding to bf16.
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + frag_col;
+      const float b0 = __bfloat162float(bias_t[c]), b1 = __bfloat162float(bias_t[c + 1]);
+      acc[4 * j] = __fadd_rn(acc[4 * j], b0); acc[4 * j + 1] = __fadd_rn(acc[4 * j + 1], b1);
+      acc[4 * j + 2] = __fadd_rn(acc[4 * j + 2], b0); acc[4 * j + 3] = __fadd_rn(acc[4 * j + 3], b1);
+    }
+    if constexpr (EPI == EPI_BF16 || EPI == EPI_F32) {   // one branch per tile
+      switch (g.act) {
+        case ACT_GELU:
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = gelu_erf(acc[i]);
+          break;
+        case ACT_RELU:
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = fmaxf(acc[i], 0.f);
+          break;
+        case ACT_SILU:
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = silu(acc[i]);
+          break;
+        case ACT_QUICKGELU:
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = acc[i] / (1.f + __expf(-1.702f * acc[i]));
+          break;
+        default: break;
+      }
+    }
+    bool keep0 = true, keep1 = true;               // row mask of the thread's two rows
+    if (g.row_keep) { keep0 = keep_t[cw * 16 + lr] != 0; keep1 = keep_t[cw * 16 + lr + 8] != 0; }
+
+    // Output box bi of the staging (16 rows x 128 B) to columns col0.. of C.  TMA writes the columns of a row in 16-byte
+    // runs, so a box that ends inside the 16-byte run holding C's last column (n_out * E not a multiple of 16) would
+    // write past it: such a box -- only ever a tile's last -- goes element by element, read by the lanes before the
+    // barrier that closes the tile.
+    constexpr int E = EPI == EPI_F32 ? 4 : 2;
+    auto put_box = [&](int bi, int col0) {
+      if ((n_out * E) % 16 == 0 || col0 + 128 / E <= n_out) {
+        if (lane == 0) tc::tma_store_2d(&tmap_c, s_buf_u32 + bi * EPI_BUF, col0, warp_row0);
+        return;
+      }
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {               // lane: 16 bytes of row rr
+        const int rr = it * 4 + (lane >> 3), piece = lane & 7, row = warp_row0 + rr;
+        if (row >= g.M) continue;
+#pragma unroll
+        for (int e = 0; e < 16 / E; ++e) {
+          const int col = col0 + piece * (16 / E) + e;
+          if (col >= n_out) break;
+          const uint8_t* sp = s_buf + bi * EPI_BUF + swz(rr, 16 * piece + E * e);
+          uint8_t* dp = reinterpret_cast<uint8_t*>(g.C) + ((size_t)row * g.ldc + col) * E;
+          if constexpr (E == 4) *reinterpret_cast<uint32_t*>(dp) = *reinterpret_cast<const uint32_t*>(sp);
+          else *reinterpret_cast<uint16_t*>(dp) = *reinterpret_cast<const uint16_t*>(sp);
+        }
+      }
+    };
+
+    if (warp_live) {
+#pragma unroll
+      for (int u = 0; u < UNITS; ++u) {
+        if (oc0 + 64 * u >= n_out) break;                      // uniform: the tile's last units lie past N
+        const int b = EPI == EPI_F32 ? 0 : (u & 1);
+        uint8_t* buf = s_buf + b * EPI_BUF;
+        if (has_res) {
+          // refill: the unit RES_AHEAD - 1 ahead goes to the buffer the previous unit's store has read
+          if (u > 0 && u + RES_AHEAD - 1 < UNITS && oc0 + 64 * (u + RES_AHEAD - 1) < n_out && lane == 0) {
+            tc::bulk_wait_read<0>();
+            load_res(u + RES_AHEAD - 1);
+          }
+          tc::mbar_wait(res_bar(2 * cw + b), (res_phase >> b) & 1);
+          res_phase ^= 1u << b;
+        } else if constexpr (EPI != EPI_SCATTER && EPI != EPI_F32) {
+          // the buffer's last store (two units back, or the previous tile's) has read it; the newest may still run
+          if (lane == 0) { if (u == 0) tc::bulk_wait_read<0>(); else tc::bulk_wait_read<1>(); }
+          __syncwarp();
+        }
+        if constexpr (EPI == EPI_SWIGLU) {
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {                    // output column 4 jj + lane % 4 of the unit
+            const int j = 16 * u + jj;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint8_t* p = buf + swz(lr + 8 * h, 16 * (jj >> 1)) + 8 * (jj & 1) + 2 * (lane & 3);
+              float o = __fmul_rn(silu(acc[4 * j + 2 * h]), acc[4 * j + 2 * h + 1]);
+              if (has_res) o = __fadd_rn(o, __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p)));
+              *reinterpret_cast<__nv_bfloat16*>(p) = __float2bfloat16(o);
+            }
+          }
         } else {
-          v0 += __bfloat162float(rp[0]);
-        }
-      }
-      if (g.row_keep && !g.row_keep[row]) { v0 = 0.f; v1 = 0.f; }
-    };
-    // destination of an output row: C, or the peer slot that owns row block d of C (scatter mode)
-    auto out_row = [&](int row) -> __nv_bfloat16* {
-      if constexpr (EPI != EPI_SCATTER) return reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc;
-      const int d = row / g.sc_rows;
-      return reinterpret_cast<__nv_bfloat16*>(g.sc_dst[d]) + (size_t)(row - d * g.sc_rows) * g.ldc;
-    };
-    // general path: the pair goes straight from the fragment to global memory (fp32 output, SwiGLU, ragged N)
-    auto emit = [&](int row, int c, float v0, float v1) {
-      const int col = n0 + c;
-      if (row >= g.M || col >= g.N) return;
-      if (swiglu) {                                  // columns (2j, 2j+1) = (gate, up) -> output column j
-        const int oc = col >> 1;
-        float o = silu(v0 + s_bias[c]) * (v1 + s_bias[c + 1]);
-        if (g.residual) o += __bfloat162float(g.residual[(size_t)row * g.ldr + oc]);
-        reinterpret_cast<__nv_bfloat16*>(g.C)[(size_t)row * g.ldc + oc] = __float2bfloat16(o);
-        return;
-      }
-      math(row, c, v0, v1);
-      const bool pair = col + 1 < g.N;               // 4-byte (bf16) / 8-byte (fp32) aligned
-      if (g.out_f32) {
-        float* cp = reinterpret_cast<float*>(g.C) + (size_t)row * g.ldc + col;
-        if (pair) *reinterpret_cast<float2*>(cp) = make_float2(v0, v1); else cp[0] = v0;
-        return;
-      }
-      __nv_bfloat16* cp = out_row(row) + col;
-      if (pair) *reinterpret_cast<__nv_bfloat162*>(cp) = __floats2bfloat162_rn(v0, v1); else cp[0] = __float2bfloat16(v0);
-    };
-    const int row0 = tm * BM + frag_row;
-    const int warp_row0 = tm * BM + wg * 64 + (warp & 3) * 16;
-    uint8_t* my_stage = s_epi + (warp - 4) * EPI_WARP_BYTES;
-    // n8 block j (columns 8j..8j+7 of the tile) is acc[4j..4j+3]
+          // *scale -> +residual -> row mask, in place in acc; EPI_BF16 / EPI_SCATTER write the pair back over its residual
 #pragma unroll
-    for (int ch = 0; ch < BN / 64; ++ch) {           // 64-column chunks of the tile
-      const int c0 = ch * 64;
-      if (n0 + c0 >= g.N) break;                     // uniform
-      if constexpr (EPI == EPI_GENERAL) {
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * u + jj, c = 8 * j + frag_col;
+            const float s0 = __bfloat162float(scale_t[c]), s1 = __bfloat162float(scale_t[c + 1]);
 #pragma unroll
-        for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
-          const int c = 8 * j + frag_col;
-          emit(row0, c, acc[4 * j], acc[4 * j + 1]);
-          emit(row0 + 8, c, acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      } else {
-        // bf16: the warp stages its 16 rows x 64 columns in shared memory, then stores 128-byte row runs
-        // (4-byte stores from the fragments would cost the L2 eight requests per 128-byte line instead of one)
+            for (int h = 0; h < 2; ++h) {
+              float& v0 = acc[4 * j + 2 * h];
+              float& v1 = acc[4 * j + 2 * h + 1];
+              uint8_t* p = buf + swz(lr + 8 * h, 16 * jj) + 4 * (lane & 3);
+              v0 = __fmul_rn(v0, s0); v1 = __fmul_rn(v1, s1);
+              if (has_res) {
+                const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+                v0 = __fadd_rn(v0, f.x); v1 = __fadd_rn(v1, f.y);
+              }
+              if (!(h ? keep1 : keep0)) { v0 = 0.f; v1 = 0.f; }
+              if constexpr (EPI != EPI_F32) *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(v0, v1);
+            }
+          }
+          if constexpr (EPI == EPI_F32) {
+            // 32 fp32 columns per buffer: every lane has read its residual from buffer 0, and both buffers' last
+            // stores have read them, before any lane overwrites them
+            if (lane == 0) tc::bulk_wait_read<0>();
+            __syncwarp();
 #pragma unroll
-        for (int j = 8 * ch; j < 8 * ch + 8; ++j) {
-          const int c = 8 * j + frag_col;
-          float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
-          math(row0, c, a0, a1);
-          math(row0 + 8, c, b0, b1);
-          const int off = (8 * (j - 8 * ch) + frag_col) * 2;
-          *reinterpret_cast<__nv_bfloat162*>(my_stage + (lane >> 2) * EPI_PITCH + off) = __floats2bfloat162_rn(a0, a1);
-          *reinterpret_cast<__nv_bfloat162*>(my_stage + ((lane >> 2) + 8) * EPI_PITCH + off) = __floats2bfloat162_rn(b0, b1);
-        }
-        __syncwarp();
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * u + jj;
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {             // each instruction: 4 rows x 128 contiguous bytes
-          const int rr = it * 4 + (lane >> 3), piece = lane & 7;
-          const uint4 val = *reinterpret_cast<const uint4*>(my_stage + rr * EPI_PITCH + piece * 16);
-          if (warp_row0 + rr < g.M) *reinterpret_cast<uint4*>(out_row(warp_row0 + rr) + n0 + c0 + piece * 8) = val;
+              for (int h = 0; h < 2; ++h) {
+                uint8_t* p = s_buf + (jj >> 2) * EPI_BUF + swz(lr + 8 * h, 32 * (jj & 3) + 8 * (lane & 3));
+                *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+              }
+            }
+          }
         }
-        __syncwarp();
+        if constexpr (EPI == EPI_SCATTER) {
+          // 16-byte stores of 128-byte row runs to the peer slot that owns row block d of C (a tile's rows share it)
+          __syncwarp();
+          const int d = warp_row0 / g.sc_rows;
+          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.sc_dst[d]) + (size_t)(warp_row0 - d * g.sc_rows) * g.ldc + n0 + 64 * u;
+#pragma unroll
+          for (int it = 0; it < 4; ++it) {             // each instruction: 4 rows x 128 contiguous bytes
+            const int rr = it * 4 + (lane >> 3), piece = lane & 7;
+            const uint4 val = *reinterpret_cast<const uint4*>(buf + swz(rr, 16 * piece));
+            *reinterpret_cast<uint4*>(dst + (size_t)rr * g.ldc + piece * 8) = val;
+          }
+          __syncwarp();                                // the buffer is read before the unit two ahead rewrites it
+        } else {
+          // every lane's generic writes to the buffer(s) are ordered before the TMA store reads them
+          tc::fence_proxy_async_smem();
+          __syncwarp();
+          if constexpr (EPI == EPI_F32) {
+            put_box(0, n0 + 64 * u);
+            if (n0 + 64 * u + 32 < n_out) put_box(1, n0 + 64 * u + 32);
+          } else {
+            put_box(b, oc0 + 64 * u);
+          }
+          if (lane == 0) tc::bulk_commit();            // one group per unit (empty when both boxes went by put_tail)
+        }
       }
     }
     if constexpr (EPI == EPI_SCATTER) {                                 // tile pushed: publish it to the owner of these rows
       __threadfence_system();
       __syncwarp();
-      if (lane == 0 && warp_row0 < g.M)
+      if (lane == 0 && warp_live)
         asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(g.sc_flag[warp_row0 / g.sc_rows]), "r"(1u) : "memory");
     }
-    tc::named_bar_sync(1, CONSUMER_THREADS);         // every reader of s_bias / s_scale is done: the next tile may overwrite
+    tc::named_bar_sync(1, CONSUMER_THREADS);         // every reader of s_bias / s_scale / s_keep is done: the next tile may overwrite
   }
+  // the bulk stores read shared memory and write C after their issue: both finish before the CTA exits
+  if (EPI != EPI_SCATTER && lane == 0) tc::bulk_wait<0>();
 }
 
 // SM budgets (0 = every SM): a persistent GEMM CTA owns its SM (384 threads with the whole register file between them), so a
@@ -357,7 +485,7 @@ int g_sm_limit = 0, g_scatter_sm_limit = 0;
 // tile (tests and sweeps).  The scatter GEMM always uses 128 x 256: its receivers count arrivals per such tile.
 int g_gemm_variant = VLLM_GEMM_DEFAULT;
 
-using KernelFn = void (*)(const CUtensorMap, const CUtensorMap, const GemmArgs);
+using KernelFn = void (*)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmArgs);
 
 // The instantiation of a launch: operand layouts from g.a_mn / g.b_mn, epilogue from the store kind (see EPI_*).
 template <int BN, int TA, int TB>
@@ -366,7 +494,11 @@ KernelFn pick_epilogue(const GemmArgs& g) {
     if constexpr (BN == 256 && !TA && !TB) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_SCATTER>;
     return nullptr;
   }
-  if (g.act == ACT_SWIGLU || g.out_f32 || g.N % 64) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_GENERAL>;
+  if (g.act == ACT_SWIGLU) {                         // only vllm_gemm_bf16, K-major operands
+    if constexpr (!TA && !TB) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_SWIGLU>;
+    return nullptr;
+  }
+  if (g.out_f32) return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_F32>;
   return gemm_bf16_wgmma_kernel<BN, TA, TB, EPI_BF16>;
 }
 template <int BN>
@@ -382,13 +514,21 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
   CUtensorMap ta, tb;
   const uint64_t nb = g.bt_rows ? (uint64_t)(g.M / g.bt_rows) : 1;     // matrices in the stack (batched mode)
   const uint64_t m_local = g.bt_rows ? (uint64_t)g.bt_rows : (uint64_t)g.M;
-  int rc = g.a_mn ? vllm_make_tmap_bf16(&ta, A, nb * (uint64_t)g.K, m_local, (uint64_t)lda, 64)       // [K, M] rows, 64 x 64 boxes
-                  : vllm_make_tmap_bf16(&ta, A, (uint64_t)(a_rows < 0 ? g.M : a_rows),
+  int rc = g.a_mn ? vllm_make_tmap_2d(&ta, A, nb * (uint64_t)g.K, m_local, (uint64_t)lda, 64)       // [K, M] rows, 64 x 64 boxes
+                  : vllm_make_tmap_2d(&ta, A, (uint64_t)(a_rows < 0 ? g.M : a_rows),
                                         (uint64_t)(a_cols < 0 ? g.K : a_cols), (uint64_t)lda, BM);
   if (rc) return rc;
-  rc = g.b_mn ? vllm_make_tmap_bf16(&tb, B, nb * (uint64_t)g.K, (uint64_t)g.N, (uint64_t)ldb, 64)
-              : vllm_make_tmap_bf16(&tb, B, nb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, BN);
+  rc = g.b_mn ? vllm_make_tmap_2d(&tb, B, nb * (uint64_t)g.K, (uint64_t)g.N, (uint64_t)ldb, 64)
+              : vllm_make_tmap_2d(&tb, B, nb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, BN);
   if (rc) return rc;
+  // the output and the residual in 16-row x 128-byte boxes (one staging buffer); the scatter GEMM stores to its peers directly
+  CUtensorMap tc_{}, tr{};
+  if (!g.sc_rows) {
+    const uint64_t n_out = (uint64_t)(g.act == ACT_SWIGLU ? g.N / 2 : g.N);
+    rc = vllm_make_tmap_2d(&tc_, g.C, (uint64_t)g.M, n_out, (uint64_t)g.ldc, 16, g.out_f32 != 0);
+    if (!rc && g.residual) rc = vllm_make_tmap_2d(&tr, g.residual, (uint64_t)g.M, n_out, (uint64_t)g.ldr, 16);
+    if (rc) return rc;
+  }
   g.tiles_m = (g.M + BM - 1) / BM;
   g.tiles_n = (g.N + BN - 1) / BN;
   const int n_tiles = g.tiles_m * g.tiles_n;
@@ -403,22 +543,23 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
   if (!kern) return VLLM_EUNSUPPORTED;
   const cudaError_t e = vllm_smem_optin(kern, C_::SMEM);
   if (e != cudaSuccess) return (int)e;
-  kern<<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, g);
+  kern<<<ctas, THREADS, C_::SMEM, st>>>(ta, tb, tc_, tr, g);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }
 
-// Default tile width of a dense K-major GEMM: 128 x 256 when the output is narrow (N <= 4096) and K is long (>= 3072),
-// else 128 x 128.  tools/gemm_bench.py, TFLOP/s 128 x 128 / 128 x 256, each shape with its model epilogue (H100 80GB
-// HBM3, 700 W power limit, median of 3):
-//   wide:   ViT proj 41000x3200x3200 370 / 409, fc2 41000x3200x12800 443 / 572, LLM down 12288x4096x11008 472 / 543,
-//           LLM o 12288x4096x4096 424 / 409 (a tie within the spread)
-//   narrow: ViT qkv 41000x9600x3200 594 / 430, fc1 (GELU) 41000x12800x3200 533 / 259, LLM qkv 12288^2x4096 558 / 439,
-//           gate|up (SwiGLU) 12288x22016x4096 537 / 420, lm_head (fp32) 12288x32026x4096 582 / 312,
-//           GDINO FFN 174080x2048x256 133 / 63, 8192^3 611 / 517
-// MN-major, batched and implicit-convolution launches were not measured at the wide tile and keep 128 x 128.
+// Default tile width of a dense K-major GEMM: 128 x 256 when N >= 2048, else 128 x 128.  tools/gemm_bench.py, TFLOP/s
+// 128 x 128 / 128 x 256 (median of 3 +- spread), each shape with its model epilogue (H100 80GB HBM3, 700 W power limit):
+//   wide ahead:  LLM down 12288x4096x11008 536+-41 / 687+-8, lm_head (fp32) 12288x32026x4096 586+-9 / 648+-36,
+//                gate|up (SwiGLU) 12288x22016x4096 598+-67 / 671+-7, GDINO FFN 174080x2048x256 298+-3 / 330+-4,
+//                ViT qkv 41000x9600x3200 629+-15 / 673+-54
+//   within the spread:  ViT proj 41000x3200x3200 620 / 613, fc1 (GELU) 41000x12800x3200 600 / 596,
+//                fc2 41000x3200x12800 620 / 630, LLM qkv 12288^2x4096 684 / 692, LLM o 12288x4096x4096 581 / 570,
+//                8192^3 666 / 656
+// Narrower outputs, MN-major, batched and implicit-convolution launches were not measured at the wide tile and keep
+// 128 x 128.
 bool wide_by_shape(const GemmArgs& g) {
-  return !g.a_mn && !g.b_mn && !g.bt_rows && !g.a_seg_kb && g.N <= 4096 && g.K >= 3072;
+  return !g.a_mn && !g.b_mn && !g.bt_rows && !g.a_seg_kb && g.N >= 2048;
 }
 
 int launch_gemm_auto(const void* A, int lda, const void* B, int ldb, const GemmArgs& g, cudaStream_t st, long long a_rows = -1,

@@ -58,6 +58,34 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+// 2-D tile store this CTA's smem -> global (bulk-group completion); elements outside the tensor map's bounds are not written
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the N most recent bulk groups of this thread have finished reading their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// all but the N most recent bulk groups of this thread are complete (their global writes done)
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// orders this thread's generic-proxy shared-memory accesses before later async-proxy (TMA) accesses
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- cp.async (LDGSTS) ---------------------------------------------------------
+// Word i of bytes [b0, b0 + n) of the global vector v (len bytes) to shared memory, in 4-byte words of the aligned grid:
+// word i is the aligned word (v + b0) / 4 * 4 + 4 i, so byte b0 + x of v lands at dst + ((v + b0) & 3) + x for x < n when
+// the caller issues words 0 .. n / 4.  Bytes at or past v + len are zero-filled and never read.  When v + b0 is not
+// 4-byte aligned, word 0 also reads the bytes in front of it within that aligned word: inside v when b0 > 0, and in
+// v's own allocation otherwise (allocations are at least 4-byte aligned).  Completes at cp_async_wait_all().
+__device__ __forceinline__ void cp_async_vec_word(uint32_t dst, const void* v, long long len, long long b0, int i) {
+  const uintptr_t base = reinterpret_cast<uintptr_t>(v);
+  const uintptr_t w = ((base + b0) & ~uintptr_t(3)) + 4u * i;
+  const long long left = (long long)(base + len) - (long long)w;
+  const int n = left >= 4 ? 4 : left > 0 ? (int)left : 0;
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst + 4u * i), "l"(w), "r"(n) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ---- register budget (warp-specialised kernels: the producer warpgroup gives registers to the consumers) ----
 template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
@@ -201,17 +229,19 @@ static inline PFN_cuTensorMapEncodeTiled_v12000 vllm_tma_encoder() {
   }
   return fn;
 }
-// bf16 matrix [rows, cols] with row pitch `ld` elements; box = [box_rows, 64 cols] (128 B), 128B swizzle.
-static inline int vllm_make_tmap_bf16(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
-                                      uint32_t box_rows) {
+// matrix [rows, cols] of bf16 (f32 = false) or fp32 elements with row pitch `ld` elements; box = [box_rows, 128 B of
+// columns] (64 bf16 / 32 fp32), 128B swizzle.  Loads fill elements outside [rows, cols] with zeros; stores skip them.
+static inline int vllm_make_tmap_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
+                                    uint32_t box_rows, bool f32 = false) {
   PFN_cuTensorMapEncodeTiled_v12000 enc = vllm_tma_encoder();
   if (!enc) return -100;
+  const uint32_t elt = f32 ? 4 : 2;
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {64, box_rows};
+  cuuint64_t strides[1] = {ld * elt};
+  cuuint32_t box[2] = {128 / elt, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base),
+                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : -101;
 }
