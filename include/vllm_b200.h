@@ -412,6 +412,22 @@ int vllm_gemm_bf16_tn(const void* A, int lda, int a_mn_major, const void* B, int
  * M % 256 == 0 (and K % 64 == 0 with MN-major operands) so tiles never straddle two matrices. */
 int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc,
                            int n_batch, int M, int N, int K, int causal, int out_f32, void* stream);
+/* Grouped batching for grouped-query attention (`group` query heads share one KV head; q head i of a batch row belongs to
+ * KV head i / group, so "B index = A index / group" and "reduce over `group` consecutive matrices" hold across the batch):
+ *   reduce = 0 (broadcast): C and A have n_batch matrices, B has n_batch / group; output matrix i = A_i . B_{i / group}^T.
+ *            causal 0 / 1 / 2 / 3 as in vllm_gemm_bf16_batched (S = Q K^T, dP = dO V^T with 1, dQ = dS K with 3).
+ *   reduce = 1: A and B have n_batch matrices, C has n_batch / group; output matrix j = sum over g < group of
+ *            A_{j group + g} . B_{j group + g}^T, accumulated in fp32 and rounded once (dV = sum_g P_g^T dO_g,
+ *            dK = sum_g dS_g^T Q_g).  Both operands MN-major: the reduction is one K axis of group * K rows.  causal 0,
+ *            or 2: the K range of every one of the group's segments starts at the tile's first row (K == M required).
+ * vllm_gemm_bf16_batched is the group = 1 broadcast.  Returns, with nothing launched:
+ *   VLLM_EINVAL        group <= 0, n_batch % group, reduce not 0 / 1, reduce with causal 1 / 3, causal 2 / 3 with K != M,
+ *                      and the size / pitch rules of vllm_gemm_bf16_batched;
+ *   VLLM_EUNSUPPORTED  reduce with a K-major operand, M % 256, K % 64 with an MN-major operand, a stack over 2^31 rows;
+ *   VLLM_EALIGN        bases not 16-byte aligned, pitches not 16-byte multiples. */
+int vllm_gemm_bf16_batched_grouped(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C,
+                                   int ldc, int n_batch, int group, int reduce, int M, int N, int K, int causal, int out_f32,
+                                   void* stream);
 /* Row kernels of the training-side path (csrc/train_ops.cu): RMSNorm backward (dx bf16, dweight fp32 ACCUMULATED --
  * zero it first), SwiGLU forward / backward on the interleaved (gate, up) columns of the gate|up GEMM, the causal
  * softmax / softmax-backward of the materialised attention backward (in place on [n_mat*T, T] bf16 stacks), and the
@@ -425,6 +441,13 @@ int vllm_rmsnorm_bwd_bf16(const void* x, long long ldx, const void* weight, cons
  * One pass of 16-byte vectors; contiguous tensors. */
 int vllm_head_stack_bf16(const void* src, void* dst, int batch, int tokens, int parts, int heads, int head_dim,
                          int to_stacked, void* stream);
+/* Grouped-query form: packed projection rows [batch, tokens, (nq + 2 nkv) head_dim] bf16 with row pitch ld elements (q heads,
+ * then k heads, then v heads) -> Q [batch, nq, tokens, head_dim], K / V [batch, nkv, tokens, head_dim] (contiguous stacks
+ * for vllm_gemm_bf16_batched_grouped) when to_stacked != 0, the inverse (stacked gradients -> packed d(qkv)) otherwise.
+ * The pitch gap of a packed row is neither read nor written.  nq % nkv != 0 or ld < (nq + 2 nkv) head_dim: VLLM_EINVAL;
+ * head_dim % 8: VLLM_EUNSUPPORTED; ld % 8 or a base not 16-byte aligned: VLLM_EALIGN. */
+int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int nq, int nkv,
+                             int head_dim, int to_stacked, void* stream);
 /* The same backward with the dweight reduction done through a workspace instead of atomics: every CTA writes its partial
  * column sums to one row of partials [n_partials >= vllm_rmsnorm_bwd_partials(rows), cols] (fp32, 16-byte aligned) and a
  * second kernel sums the rows in order -- deterministic (the atomic form puts ~1200 atomics on each of the 4096 column

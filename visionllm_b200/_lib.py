@@ -51,8 +51,10 @@ _SIGNATURES = {
     "vllm_conv_rows_bf16": (ci, [vp, cll, ci, ci, ci, ci, vp, ci, vp, ci, ci, vp, ci, vp]),
     "vllm_gemm_bf16_tn": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, vp]),
     "vllm_gemm_bf16_batched": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
+    "vllm_gemm_bf16_batched_grouped": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_rmsnorm_bwd_bf16": (ci, [vp, cll, vp, vp, cll, vp, cll, vp, cll, ci, cf, vp]),
     "vllm_head_stack_bf16": (ci, [vp, vp, ci, ci, ci, ci, ci, ci, vp]),
+    "vllm_head_stack_qkv_bf16": (ci, [vp, cll, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_rmsnorm_bwd_partials": (ci, [cll]),
     "vllm_rmsnorm_bwd_ws_bf16": (ci, [vp, cll, vp, vp, cll, vp, cll, vp, vp, ci, cll, ci, cf, vp]),
     "vllm_swiglu_fwd_bf16": (ci, [vp, cll, vp, cll, cll, ci, vp]),

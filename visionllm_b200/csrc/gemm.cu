@@ -29,7 +29,7 @@
 // Instantiations gemm_bf16_wgmma_kernel<BN, TA, TB, EPI> (chosen per launch by pick_kernel, 19 in all):
 //   BN  128 | 256            tile width (vllm_gemm_set_variant; the scatter GEMM is always 256)
 //   TA, TB  0 | 1            K-major | MN-major operand: (0, 0) for every forward call, the other three for
-//                            vllm_gemm_bf16_tn / _batched (training)
+//                            vllm_gemm_bf16_tn / _batched / _batched_grouped (training)
 //   EPI  EPI_BF16 | EPI_F32 for every (BN, TA, TB); EPI_SWIGLU for <BN, 0, 0>; EPI_SCATTER only for <256, 0, 0>
 // The layout is a template parameter so that the k-block (fence, four MMAs, commit, wait) is one basic block: with a
 // run-time layout branch inside it, ptxas closes the wgmma group in each branch and the wait after the join retires
@@ -76,16 +76,26 @@ struct GemmArgs {
   // strictly above the diagonal (S = Q K^T, dP = dO V^T), 2 = the K range starts at the tile's first row (dV = P^T dO,
   // dK = dS^T Q: P, dS are zero below), 3 = the K range ends at the tile's last row (dQ = dS K).
   int bt_rows, causal;
+  // Grouped batching (vllm_gemm_bf16_batched_grouped: grouped-query attention, `group` query heads per KV head).
+  // reduce = 0 (broadcast): output matrix i meets A matrix i and B matrix i / group.  reduce = 1: output matrix j is the
+  // sum over g < group of A_{j group + g} . B_{j group + g}^T -- both operands MN-major, so the group's K rows are
+  // contiguous and the K axis is `group` segments of K rows, each with the K range of the causal mode.
+  int group, reduce;
 };
 
-// per-tile K range / operand offsets of the batched mode (identity when bt_rows == 0)
-struct TilePlan { int skip, kb0, kb1, b_row_off, k_off; };
+// Per-tile K range and operand offsets of the batched mode (identity when bt_rows == 0): the tile reads `segs` segments,
+// k-blocks kb0 .. kb1 - 1 of each; segment s of an MN-major operand starts s * K rows after its k offset.
+struct TilePlan { int skip, kb0, kb1, segs, b_row_off, a_k_off, b_k_off; };
 __device__ __forceinline__ TilePlan plan_tile(const GemmArgs& g, int m0, int n0, int rows_per_tile, int num_kb) {
-  TilePlan p{0, 0, num_kb, 0, 0};
+  TilePlan p{0, 0, num_kb, 1, 0, 0, 0};
   if (g.bt_rows) {
     const int bh = m0 / g.bt_rows, ml = m0 - bh * g.bt_rows;
-    p.b_row_off = bh * g.N;                             // K-major B: a stack of [N, K] matrices along the rows
-    p.k_off = bh * g.K;                                 // MN-major operands: stacks of [K, M|N] matrices along the K rows
+    const int a_mat = g.reduce ? bh * g.group : bh;     // first A / B matrix the output matrix bh meets
+    const int b_mat = g.reduce ? bh * g.group : bh / g.group;
+    p.segs = g.reduce ? g.group : 1;
+    p.b_row_off = b_mat * g.N;                          // K-major B: a stack of [N, K] matrices along the rows
+    p.a_k_off = a_mat * g.K;                            // MN-major operands: stacks of [K, M|N] matrices along the K rows
+    p.b_k_off = b_mat * g.K;
     if (g.causal == 1 && n0 >= ml + rows_per_tile) p.skip = 1;
     if (g.causal == 2) p.kb0 = ml / BK;
     if (g.causal == 3) { const int e = (ml + rows_per_tile + BK - 1) / BK; p.kb1 = e < num_kb ? e : num_kb; }
@@ -209,29 +219,31 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         // K-major A: global stacked row; MN-major A: column inside its matrix (the stack runs along the K rows)
         const int row_a = tm * BM - (TA ? bt_m0 : 0);
         const int row_b = tn * BN + (TB ? 0 : tp.b_row_off);
-        const int ka_off = TA ? tp.k_off : 0, kb_off = TB ? tp.k_off : 0;
-        for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
-          tc::mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t sa = smem_base + stage * C_::STAGE_BYTES, sb = sa + A_BYTES;
-          int ka = kb * BK + ka_off, ra = row_a;
-          if (g.a_seg_kb) {
-            const int seg = kb / g.a_seg_kb;
-            ka = (kb - seg * g.a_seg_kb) * BK;
-            ra = row_a + seg * g.a_seg_rows;
+        for (int gs = 0; gs < tp.segs; ++gs) {            // grouped reduce: one segment per matrix of the group
+          const int ka_off = TA ? tp.a_k_off + gs * g.K : 0, kb_off = TB ? tp.b_k_off + gs * g.K : 0;
+          for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
+            tc::mbar_wait(empty_bar(stage), phase ^ 1);
+            const uint32_t sa = smem_base + stage * C_::STAGE_BYTES, sb = sa + A_BYTES;
+            int ka = kb * BK + ka_off, ra = row_a;
+            if (g.a_seg_kb) {
+              const int seg = kb / g.a_seg_kb;
+              ka = (kb - seg * g.a_seg_kb) * BK;
+              ra = row_a + seg * g.a_seg_rows;
+            }
+            tc::mbar_arrive_expect_tx(full_bar(stage), C_::STAGE_BYTES);
+            if constexpr (TA) {
+              for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
+            } else {
+              tc::tma_load_2d(sa, &tmap_a, full_bar(stage), ka, ra);
+            }
+            if constexpr (TB) {
+              for (int h = 0; h < BN / 64; ++h)
+                tc::tma_load_2d(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
+            } else {
+              tc::tma_load_2d(sb, &tmap_b, full_bar(stage), kb * BK, row_b);
+            }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-          tc::mbar_arrive_expect_tx(full_bar(stage), C_::STAGE_BYTES);
-          if constexpr (TA) {
-            for (int h = 0; h < BM / 64; ++h) tc::tma_load_2d(sa + h * 8192, &tmap_a, full_bar(stage), ra + 64 * h, ka);
-          } else {
-            tc::tma_load_2d(sa, &tmap_a, full_bar(stage), ka, ra);
-          }
-          if constexpr (TB) {
-            for (int h = 0; h < BN / 64; ++h)
-              tc::tma_load_2d(sb + h * 8192, &tmap_b, full_bar(stage), row_b + 64 * h, kb * BK + kb_off);
-          } else {
-            tc::tma_load_2d(sb, &tmap_b, full_bar(stage), kb * BK, row_b);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -291,10 +303,11 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         if (oc0 + 64 * u < n_out) load_res(u);
     }
     int prev_stage = -1;
-    for (int kb = tp.kb0; kb < tp.kb1; ++kb) {
+    const int n_kb = tp.segs * (tp.kb1 - tp.kb0);     // the producer's k-blocks of this tile, segment after segment
+    for (int kb = 0; kb < n_kb; ++kb) {
       tc::mbar_wait(full_bar(stage), phase);
       const uint32_t sa = smem_base + stage * C_::STAGE_BYTES + wg * 8192, sb = smem_base + stage * C_::STAGE_BYTES + A_BYTES;
-      const bool first = kb == tp.kb0;
+      const bool first = kb == 0;
       tc::acc_fence(acc);
       tc::wgmma_fence();
       mma_kblock<BN, TA, TB>(acc, sa, sb, first);
@@ -512,14 +525,18 @@ int launch_gemm(const void* A, int lda, const void* B, int ldb, GemmArgs g, cuda
                 int a_cols = -1) {
   using C_ = Cfg<BN>;
   CUtensorMap ta, tb;
-  const uint64_t nb = g.bt_rows ? (uint64_t)(g.M / g.bt_rows) : 1;     // matrices in the stack (batched mode)
+  // matrices in each stack (batched mode): C has nb; A has nb (broadcast) or nb * group (reduce); B has nb / group or
+  // nb * group
+  const uint64_t nb = g.bt_rows ? (uint64_t)(g.M / g.bt_rows) : 1;
+  const uint64_t na = g.bt_rows && g.reduce ? nb * g.group : nb;
+  const uint64_t nbb = !g.bt_rows ? 1 : g.reduce ? nb * g.group : nb / g.group;
   const uint64_t m_local = g.bt_rows ? (uint64_t)g.bt_rows : (uint64_t)g.M;
-  int rc = g.a_mn ? vllm_make_tmap_2d(&ta, A, nb * (uint64_t)g.K, m_local, (uint64_t)lda, 64)       // [K, M] rows, 64 x 64 boxes
+  int rc = g.a_mn ? vllm_make_tmap_2d(&ta, A, na * (uint64_t)g.K, m_local, (uint64_t)lda, 64)       // [K, M] rows, 64 x 64 boxes
                   : vllm_make_tmap_2d(&ta, A, (uint64_t)(a_rows < 0 ? g.M : a_rows),
                                         (uint64_t)(a_cols < 0 ? g.K : a_cols), (uint64_t)lda, BM);
   if (rc) return rc;
-  rc = g.b_mn ? vllm_make_tmap_2d(&tb, B, nb * (uint64_t)g.K, (uint64_t)g.N, (uint64_t)ldb, 64)
-              : vllm_make_tmap_2d(&tb, B, nb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, BN);
+  rc = g.b_mn ? vllm_make_tmap_2d(&tb, B, nbb * (uint64_t)g.K, (uint64_t)g.N, (uint64_t)ldb, 64)
+              : vllm_make_tmap_2d(&tb, B, nbb * (uint64_t)g.N, (uint64_t)g.K, (uint64_t)ldb, BN);
   if (rc) return rc;
   // the output and the residual in 16-row x 128-byte boxes (one staging buffer); the scatter GEMM stores to its peers directly
   CUtensorMap tc_{}, tr{};
@@ -645,16 +662,20 @@ int vllm_gemm_bf16_tn(const void* A, int lda, int a_mn_major, const void* B, int
   return launch_gemm_auto(A, lda, B, ldb, g, st);
 }
 
-int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc,
-                           int n_batch, int M, int N, int K, int causal, int out_f32, void* stream) {
-  // n_batch independent products C_b[M, N] = A_b . B_b^T in ONE launch: every operand / the output is a stack of its
-  // n_batch matrices along the row axis (K-major A: [n_batch*M, K]; MN-major A: [n_batch*K, M]; same for B; C: [n_batch*M, N]).
-  // causal (square attention matrices, M == the sequence length): see GemmArgs.  The attention-backward GEMMs of a layer.
-  if (n_batch < 0 || M <= 0 || N <= 0 || K <= 0 || causal < 0 || causal > 3) return VLLM_EINVAL;
+int vllm_gemm_bf16_batched_grouped(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C,
+                                   int ldc, int n_batch, int group, int reduce, int M, int N, int K, int causal, int out_f32,
+                                   void* stream) {
+  // n_batch products A_i . B_{i / group}^T (broadcast) or n_batch / group sums of `group` products (reduce) in ONE launch;
+  // every operand / the output is a stack of its matrices along the row axis (K-major A: [n*M, K]; MN-major A: [n*K, M];
+  // same for B; C: [n*M, N]).  causal (square attention matrices, M == the sequence length): see GemmArgs.
+  if (n_batch < 0 || M <= 0 || N <= 0 || K <= 0 || causal < 0 || causal > 3 || (reduce != 0 && reduce != 1)) return VLLM_EINVAL;
+  if (group <= 0 || n_batch % group) return VLLM_EINVAL;
   if (causal >= 2 && K != M) return VLLM_EINVAL;     // modes 2 / 3 cut the K axis at the tile's rows: K is the sequence axis, and
                                                      // with K == M (a multiple of 256) every tile keeps at least one k-block
+  if (reduce && (causal == 1 || causal == 3)) return VLLM_EINVAL;   // a reduce output is a key-side gradient (dK, dV)
   if (n_batch == 0) return VLLM_OK;
   if (!A || !B || !C) return VLLM_EINVAL;
+  if (reduce && (!a_mn_major || !b_mn_major)) return VLLM_EUNSUPPORTED;   // the group's K rows are contiguous only MN-major
   if (M % 256 || ((a_mn_major || b_mn_major) && K % BK)) return VLLM_EUNSUPPORTED;     // tiles must not straddle matrices
   if ((long long)n_batch * M > 2147483647LL || (long long)n_batch * K > 2147483647LL || (long long)n_batch * N > 2147483647LL)
     return VLLM_EUNSUPPORTED;
@@ -662,11 +683,19 @@ int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B
   if (!vllm_aligned(A, 16) || !vllm_aligned(B, 16) || (lda % 8) || (ldb % 8)) return VLLM_EALIGN;
   if (!vllm_aligned(C, 16) || ((size_t)ldc * (out_f32 ? 4 : 2)) % 16) return VLLM_EALIGN;
   GemmArgs g{};
-  g.M = n_batch * M; g.N = N; g.K = K; g.C = C; g.ldc = ldc; g.out_f32 = out_f32;
+  g.M = (reduce ? n_batch / group : n_batch) * M; g.N = N; g.K = K; g.C = C; g.ldc = ldc; g.out_f32 = out_f32;
   g.a_mn = a_mn_major ? 1 : 0; g.b_mn = b_mn_major ? 1 : 0;
-  g.bt_rows = M; g.causal = causal;
+  g.bt_rows = M; g.causal = causal; g.group = group; g.reduce = reduce;
   cudaStream_t st = (cudaStream_t)stream;
   return launch_gemm_auto(A, lda, B, ldb, g, st);
+}
+
+int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C, int ldc,
+                           int n_batch, int M, int N, int K, int causal, int out_f32, void* stream) {
+  // n_batch independent products C_b[M, N] = A_b . B_b^T: the group = 1 broadcast of vllm_gemm_bf16_batched_grouped.
+  // The attention-backward GEMMs of a layer.
+  return vllm_gemm_bf16_batched_grouped(A, lda, a_mn_major, B, ldb, b_mn_major, C, ldc, n_batch, 1, 0, M, N, K, causal,
+                                        out_f32, stream);
 }
 
 int vllm_gemm_bf16_scatter(const void* A, int lda, const void* B, int ldb, void* const* dst, void* const* flags,

@@ -308,6 +308,33 @@ head_stack_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int B,
   }
 }
 
+// Grouped-query form of the same layout change: packed projection rows [B, T, (nq + 2 nkv) D] with row pitch ld_vec
+// 16-byte vectors (q heads, then k heads, then v heads) <-> three stacks Q [B, nq, T, D], K [B, nkv, T, D], V [B, nkv, T, D].
+// i indexes the concatenation Q | K | V of the stacks (coalesced on the stacked side); the pitch gap of a packed row is
+// neither read nor written.
+__global__ void __launch_bounds__(256)
+head_stack_qkv_kernel(uint4* __restrict__ packed, long long ld_vec, uint4* __restrict__ q, uint4* __restrict__ k,
+                      uint4* __restrict__ v, int B, int T, int NQ, int NKV, int DV, int to_stacked, long long n_vec) {
+  const long long n_q = (long long)B * NQ * T * DV, n_kv = (long long)B * NKV * T * DV;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (long long)gridDim.x * blockDim.x) {
+    long long r = i;
+    uint4* st = q; int heads = NQ, h0 = 0;
+    if (r >= n_q) {
+      r -= n_q;
+      if (r < n_kv) { st = k; heads = NKV; h0 = NQ; }
+      else { r -= n_kv; st = v; heads = NKV; h0 = NQ + NKV; }
+    }
+    const long long si = r;
+    const int d = (int)(r % DV); r /= DV;
+    const int t = (int)(r % T); r /= T;
+    const int h = (int)(r % heads);
+    const int b = (int)(r / heads);
+    const long long pi = ((long long)b * T + t) * ld_vec + (long long)(h0 + h) * DV + d;
+    if (to_stacked) st[si] = packed[pi];
+    else packed[pi] = st[si];
+  }
+}
+
 // logits fp32 [rows, V] (pitch ld), labels int64 [rows] (-100 = ignore), n_valid: device int64 scalar.
 // loss_sum += -log softmax(logits)[label] (fp32 atomic); dlogits bf16 [rows, V] (pitch ldd) = (softmax - onehot) / n_valid,
 // zero rows for ignored labels.  One CTA (512 threads) per row, three passes over the row (max, sum, write).
@@ -421,6 +448,26 @@ int vllm_head_stack_bf16(const void* src, void* dst, int batch, int tokens, int 
   if (blocks > cap) blocks = cap;
   head_stack_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const uint4*)src, (uint4*)dst, batch, tokens, parts,
                                                                        heads, head_dim / 8, to_stacked ? 1 : 0, n_vec);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int nq, int nkv,
+                             int head_dim, int to_stacked, void* stream) {
+  if (batch < 0 || tokens < 0 || nq <= 0 || nkv <= 0 || head_dim <= 0 || nq % nkv) return VLLM_EINVAL;
+  if (ld < (long long)(nq + 2 * nkv) * head_dim) return VLLM_EINVAL;
+  const long long n_vec = (long long)batch * tokens * (nq + 2 * nkv) * (head_dim / 8);
+  if (n_vec == 0) return VLLM_OK;
+  if (!packed || !q || !k || !v) return VLLM_EINVAL;
+  if (head_dim % 8) return VLLM_EUNSUPPORTED;
+  if (ld % 8 || !vllm_aligned(packed, 16) || !vllm_aligned(q, 16) || !vllm_aligned(k, 16) || !vllm_aligned(v, 16))
+    return VLLM_EALIGN;
+  long long blocks = (n_vec + 255) / 256;
+  const long long cap = (long long)vllm_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  head_stack_qkv_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((uint4*)packed, ld / 8, (uint4*)q, (uint4*)k,
+                                                                           (uint4*)v, batch, tokens, nq, nkv, head_dim / 8,
+                                                                           to_stacked ? 1 : 0, n_vec);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }
