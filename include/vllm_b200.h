@@ -463,6 +463,10 @@ int vllm_softmax_causal_bf16(void* s, long long ld, long long n_mat, int T, floa
 int vllm_attn_ds_bf16(const void* p, void* dp, long long ld, long long n_mat, int T, float scale, void* stream);
 int vllm_ce_loss_f32(const float* logits, long long ld, const int64_t* labels, const int64_t* n_valid, long long rows, int vocab,
                      float* loss_sum, void* dlogits, long long ldd, void* stream);
+/* x [rows, cols] bf16 (row pitch ld) *= *scale in place, the product in fp32 and rounded once; `scale` is one fp32 on the
+ * device (the upstream gradient of the loss: CrossEntropyFn.backward scales dlogits by it without a host sync).
+ * ld % 8 or a base not 16-byte aligned: VLLM_EALIGN. */
+int vllm_scale_rows_bf16(void* x, long long ld, long long rows, int cols, const float* scale, void* stream);
 
 /* ---- sequence assembly of VisionLLMv2Model.forward (SURVEY 8f rank 2, 8a-a7/a9; csrc/seqglue.cu) -----------------
  * vllm_seq_index: ONE pass over input_ids [batch, seq_len] (int64, device) producing

@@ -109,3 +109,5 @@ def test_round2_entry_points_marshal_and_accept_empty_problems():
     assert L.vllm_softmax_causal_bf16(None, 2048, 0, 2048, 0.088, None) == 0
     assert L.vllm_attn_ds_bf16(None, None, 2048, 0, 2048, 0.088, None) == 0
     assert L.vllm_ce_loss_f32(None, 32028, None, None, 0, 32026, None, None, 32032, None) == 0
+    assert L.vllm_scale_rows_bf16(None, 32032, 0, 32026, None, None) == 0
+    assert L.vllm_scale_rows_bf16(None, 32024, 4, 32026, None, None) < 0                                         # ld < cols

@@ -62,6 +62,7 @@ _SIGNATURES = {
     "vllm_softmax_causal_bf16": (ci, [vp, cll, cll, ci, cf, vp]),
     "vllm_attn_ds_bf16": (ci, [vp, vp, cll, cll, ci, cf, vp]),
     "vllm_ce_loss_f32": (ci, [vp, cll, vp, vp, cll, ci, vp, vp, cll, vp]),
+    "vllm_scale_rows_bf16": (ci, [vp, cll, cll, ci, vp, vp]),
     "vllm_gemm_set_variant": (ci, [ci]),
     "vllm_rmsnorm_bf16": (ci, [vp, cll, vp, vp, cll, cll, ci, cf, vp]),
     "vllm_layernorm_bf16": (ci, [vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),

@@ -369,6 +369,23 @@ ce_loss_kernel(const float* __restrict__ logits, long long ld, const int64_t* __
   }
 }
 
+// x [rows, cols] bf16 (pitch ld) *= *scale in place: fp32 product, one rounding; the scale is read on the device (the
+// upstream gradient of a loss, so no host sync).  One CTA per row, 16-byte vectors, the cols % 8 tail scalar.
+__global__ void __launch_bounds__(256)
+scale_rows_kernel(__nv_bfloat16* __restrict__ x, long long ld, int cols, const float* __restrict__ scale) {
+  const float s = *scale;
+  __nv_bfloat16* xr = x + (long long)blockIdx.x * ld;
+  const int nvec = cols / 8;
+  for (int v = threadIdx.x; v < nvec; v += 256) {
+    uint4* p = reinterpret_cast<uint4*>(xr) + v;
+    float f[8]; unpack8(*p, f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] *= s;
+    *p = pack8(f);
+  }
+  for (int c = nvec * 8 + threadIdx.x; c < cols; c += 256) xr[c] = __float2bfloat16(__bfloat162float(xr[c]) * s);
+}
+
 }  // namespace
 
 extern "C" {
@@ -545,6 +562,17 @@ int vllm_ce_loss_f32(const float* logits, long long ld, const int64_t* labels, c
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
   ce_loss_kernel<<<(unsigned)rows, 512, 0, (cudaStream_t)stream>>>(logits, ld, labels, n_valid, vocab, loss_sum,
                                                                    (__nv_bfloat16*)dlogits, ldd);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+int vllm_scale_rows_bf16(void* x, long long ld, long long rows, int cols, const float* scale, void* stream) {
+  if (rows < 0 || cols < 0 || ld < cols) return VLLM_EINVAL;
+  if (rows == 0 || cols == 0) return VLLM_OK;
+  if (!x || !scale) return VLLM_EINVAL;
+  if (ld % 8 || !vllm_aligned(x, 16)) return VLLM_EALIGN;
+  if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
+  scale_rows_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)x, ld, cols, scale);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }

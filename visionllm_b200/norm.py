@@ -8,7 +8,8 @@ The reference swaps its RMSNorm implementation by REBINDING A MODULE ATTRIBUTE:
 `B200RMSNorm` has FusedRMSNorm's constructor (`normalized_shape, eps, elementwise_affine`) and parameter name (`weight`),
 its forward is `vllm_rmsnorm_bf16` (fp32 statistics, x * rsqrt rounded to the input dtype THEN times weight -- the
 semantics of apex `cuApplyRMSNorm` / `manual_rms_norm`, apex/normalization/fused_layer_norm.py:16-29), and it is
-differentiable through `vllm_rmsnorm_bwd_bf16` (apex `rms_backward_affine`).  `install()` performs the same rebinding.
+differentiable through `train.RMSNormFn`, whose backward is `vllm_rmsnorm_bwd_ws_bf16` (apex `rms_backward_affine`;
+the weight gradient summed in a fixed order, so it is deterministic).  `install()` performs the same rebinding.
 """
 import numbers
 

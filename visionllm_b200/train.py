@@ -8,7 +8,8 @@ whose forward AND backward are this repo's kernels:
   op                forward                                   backward
   Linear            wgmma GEMM (ops.linear)                 dgrad / wgrad on the same kernel with MN-major operands
                                                               (ops.gemm_tn: no transposed copies of W, dy or x)
-  RMSNorm           vllm_rmsnorm_bf16                         vllm_rmsnorm_bwd_bf16 (dx + fp32 dweight)
+  RMSNorm           vllm_rmsnorm_bf16                         vllm_rmsnorm_bwd_ws_bf16 (dx + fp32 dweight, summed in
+                                                              a fixed order through per-CTA partials)
   RoPE              vllm_rope_bf16 (q and k heads)            the same kernel with -sin (the rotation's transpose)
   causal attention  wgmma flash forward (ops.attention)     materialised backward: 5 block-diagonal batched wgmma GEMMs
                                                               over all (batch, head) matrices of the layer with causal
@@ -18,7 +19,8 @@ whose forward AND backward are this repo's kernels:
                                                               matrix i / G and reduces dK / dV over the G query
                                                               matrices of a KV head inside the GEMM (no repeated K / V)
   SwiGLU            vllm_swiglu_fwd_bf16 on the gate|up GEMM  vllm_swiglu_bwd_bf16
-  CE loss           vllm_ce_loss_f32 (loss + dlogits in one pass over the fp32 logits)
+  CE loss           vllm_ce_loss_f32 (loss + dlogits in one pass over the fp32 logits); the upstream gradient
+                                                              scales dlogits in place (vllm_scale_rows_bf16)
 
 `B200LlamaForCausalLMTrain` / `B200InternLM2ForCausalLMTrain` wrap the inference module's parameters (same state dict)
 and run a fwd+bwd step; both share one per-layer loop (`decoder_layer_train`).
@@ -306,12 +308,15 @@ class SwiGLUFn(torch.autograd.Function):
 
 
 class CrossEntropyFn(torch.autograd.Function):
-    """mean CE over labels != -100 of fp32 logits [rows, V]; loss and dlogits from one kernel."""
+    """mean CE of fp32 logits [rows, V] over the rows whose label is in [0, V) (-100 and any other label outside the
+    vocabulary are ignored, the same rows as `ops.ce_loss` and the kernel); loss and dlogits from one kernel.  When every
+    row is ignored the loss is 0 with a zero gradient (torch and `ops.ce_loss` give nan), so that a micro-batch without
+    text positions adds nothing to an accumulated step."""
 
     @staticmethod
     def forward(ctx, logits, labels):
         rows, V = logits.shape
-        n_valid = (labels >= 0).sum().to(torch.int64).reshape(1)
+        n_valid = ((labels >= 0) & (labels < V)).sum().to(torch.int64).reshape(1)
         loss_sum = torch.zeros(1, dtype=torch.float32, device=logits.device)
         # bf16 rows with a 16-byte pitch, so the lm_head dgrad / wgrad GEMMs read dlogits in place (TMA operand)
         dlogits = torch.empty((rows, (V + 7) // 8 * 8), dtype=torch.bfloat16, device=logits.device)[:, :V]
@@ -325,7 +330,13 @@ class CrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dloss):
         (dlogits,) = ctx.saved_tensors
-        dlogits.mul_(dloss.to(dlogits.dtype))                 # in place: keeps the padded pitch (dloss is 1 for a plain .backward())
+        # in place, keeping the padded pitch: dlogits * dloss in fp32 with one rounding (dloss = 1 leaves every byte as it
+        # is; a bf16 dloss would bias every gradient, e.g. by +0.2 % for bf16(1/3) under 3-way gradient accumulation)
+        scale = dloss.detach().to(torch.float32).reshape(1).contiguous()
+        rows, V = dlogits.shape
+        with torch.cuda.device(dlogits.device):
+            rc = _lib.lib().vllm_scale_rows_bf16(dlogits.data_ptr(), dlogits.stride(0), rows, V, scale.data_ptr(), _stream())
+        _check(rc, "vllm_scale_rows_bf16")
         return dlogits, None
 
 
