@@ -41,9 +41,11 @@ const char* vllm_version(void);
  * sampling_loc [batch, num_query, num_heads, num_levels, num_point, 2] (x,y);
  * attn_weight [batch, num_query, num_heads, num_levels, num_point];
  * out [batch, num_query, num_heads*channels].
- * host_shapes_hint: optional HOST copy of spatial_shapes (may be NULL); only
- * used to order the work (2-D pixel patches when num_query == spatial_size);
- * results never depend on it.
+ * host_shapes_hint: optional HOST copy of spatial_shapes (may be NULL); when given
+ * it MUST equal spatial_shapes.  It orders the work (2-D pixel patches when
+ * num_query == spatial_size) and sizes the window kernel's TMA maps; with a hint
+ * equal to spatial_shapes the result is bit-identical to the NULL-hint result.
+ * Any batch size: batches over 65535 images run as several launches.
  * flags bit0 (VLLM_MSDA_STRICT): reference thread mapping and summation order
  * with no FMA contraction -- bit-exact against oracle/msda_oracle.c.
  */
@@ -54,9 +56,12 @@ int vllm_msda_forward_f32(const float* value, const int64_t* spatial_shapes, con
                           int num_point, const int64_t* host_shapes_hint, int flags, void* stream);
 /* "Fast mode" of the same operator (SURVEY 8d cfg 2b): value is bf16 [N,S,M,32] -- the bf16 value_proj output the
  * reference upcasts with .float() before calling its fp32-only kernel (modeling_ov_grounding_dino_mask_dn.py:764-766)
- * -- sampling_loc / attn_weight stay fp32, accumulation is fp32, out is fp32 or bf16 (out_bf16) [N,Lq,M*32].  Results
- * equal vllm_msda_forward_f32 on the upcast value (bf16 -> fp32 is exact).  channels == 32, levels*points <= 32,
- * else VLLM_EUNSUPPORTED. */
+ * -- sampling_loc / attn_weight stay fp32, accumulation is fp32, out is fp32 or bf16 (out_bf16) [N,Lq,M*32].  Same
+ * products as vllm_msda_forward_f32 on the upcast value (bf16 -> fp32 is exact), summed in another order: each lane
+ * sums every second sample and a 4 + 2 + 1 shuffle tree joins them, so results are bit-identical to _f32 only for
+ * levels*points == 1 and otherwise agree within the fp32 reassociation bound of both.  A bf16 out is the fp32 result
+ * rounded to nearest.  channels == 32, levels*points <= 32, else VLLM_EUNSUPPORTED; value / out not 16-byte or
+ * sampling_loc not 8-byte aligned: VLLM_EALIGN. */
 int vllm_msda_forward_bf16v(const void* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
                             const float* sampling_loc, const float* attn_weight, void* out, int out_bf16, int batch,
                             int spatial_size, int num_heads, int channels, int num_levels, int num_query,

@@ -122,7 +122,8 @@ constexpr int MSDA_META_ROW = 32 + 2;  // int2 per corner row (32 samples + pad)
 // in place halves the bytes every sample pulls through L1 (the kernel's real bound) and drops the fp32 upcast copy
 // the reference makes (modeling_ov_grounding_dino_mask_dn.py:764).  A corner row is then 64 B = 4 x 16 B, so 16 lanes
 // cover a sample and the two half-warps take the even / odd samples: half the gather instructions per (query, head).
-// Arithmetic is unchanged (bf16 -> fp32 is exact, fp32 FMAs), so results equal the fp32 kernel on the upcast value.
+// The products are unchanged (bf16 -> fp32 is exact, fp32 FMAs) but each lane sums every second sample and a 4 + 2 + 1
+// shuffle tree joins them, so results equal the fp32 kernel on the upcast value only when K == 1.
 template <int TH, int TW, int NW, int KC, int PC, typename OutT, typename ValT = float>
 __global__ void __launch_bounds__(NW * 32)
 msda_fwd_warp_kernel(const ValT* __restrict__ value, const int64_t* __restrict__ shapes,
@@ -437,15 +438,25 @@ static int launch_warp(const ValT* value, const int64_t* shapes, const int64_t* 
                        const int64_t* host_shapes, cudaStream_t st) {
   MsdaTiling tl; memset(&tl, 0, sizeof(tl));
   build_tiling(tl, host_shapes, L, Lq, S, TH, TW);
-  dim3 grid((unsigned)(tl.n_tiles * M), (unsigned)N);
-  if (N > 65535) return VLLM_EUNSUPPORTED;
-  if (L == 4 && P == 4)
-    msda_fwd_warp_kernel<TH, TW, NW, 16, 4, OutT, ValT><<<grid, NW * 32, 0, st>>>(value, shapes, lsi, loc, attw, out,
-                                                                                  S, M, L, Lq, P, tl);
-  else
-    msda_fwd_warp_kernel<TH, TW, NW, 0, 0, OutT, ValT><<<grid, NW * 32, 0, st>>>(value, shapes, lsi, loc, attw, out, S,
-                                                                                 M, L, Lq, P, tl);
-  VLLM_CHECK_LAUNCH();
+  // the grid's y extent is the batch: larger batches run as chunks of <= 65535 images with offset pointers (the
+  // per-image arithmetic does not change, so neither do the results)
+  const int K = L * P;
+  for (int b0 = 0; b0 < N; b0 += 65535) {
+    const int nb = N - b0 < 65535 ? N - b0 : 65535;
+    const size_t img = (size_t)b0 * Lq * M;                  // (query, head) pairs before image b0
+    const ValT* v = value + (size_t)b0 * S * M * 32;
+    const float* lc = loc + img * K * 2;
+    const float* aw = attw + img * K;
+    OutT* o = out + img * 32;
+    dim3 grid((unsigned)(tl.n_tiles * M), (unsigned)nb);
+    if (L == 4 && P == 4)
+      msda_fwd_warp_kernel<TH, TW, NW, 16, 4, OutT, ValT><<<grid, NW * 32, 0, st>>>(v, shapes, lsi, lc, aw, o, S, M, L,
+                                                                                    Lq, P, tl);
+    else
+      msda_fwd_warp_kernel<TH, TW, NW, 0, 0, OutT, ValT><<<grid, NW * 32, 0, st>>>(v, shapes, lsi, lc, aw, o, S, M, L,
+                                                                                   Lq, P, tl);
+    VLLM_CHECK_LAUNCH();
+  }
   return VLLM_OK;
 }
 

@@ -20,7 +20,7 @@
 //   4. a (query, head) with a sample outside its window (ballot) re-bases that pair on global memory and takes the
 //      predicated path of msda.cu -- same arithmetic, so results do not depend on the window size.
 // Arithmetic per corner is the one of msda_fwd_warp_kernel ((row weight x column weight) x attention weight, fp32
-// FMAs): fast-mode tolerance class (<= 1e-5 max|ref| in fp32), indices bit-exact.
+// FMAs), so results are bit-identical to it; indices bit-exact (error bound: tests/test_deformable_contract_gpu.py).
 #include "msda_common.cuh"
 #include "tc_common.cuh"
 #include <string.h>

@@ -134,7 +134,8 @@ def ms_deform_attn_sample_indices(spatial_shapes, sampling_loc):
 def ms_deform_attn_forward_bf16(value, spatial_shapes, level_start_index, sampling_loc, attn_weight, out_dtype=None):
     """"Fast mode" (SURVEY 8d cfg 2b), an extension next to the reference API: value bf16 [N,S,M,32] read in place
     (the reference upcasts it with .float() first, gd.py:764), sampling_loc / attn_weight fp32, fp32 accumulation,
-    out bf16 (default) or fp32.  Equal to ms_deform_attn_forward(value.float(), ...) up to the output rounding."""
+    out bf16 (default) or fp32.  The same products as ms_deform_attn_forward(value.float(), ...) summed in another
+    order (bit-identical only for levels * points == 1), then one rounding to the output dtype."""
     N, S, M, D, L, Lq, P = _check_inputs(
         value, spatial_shapes, level_start_index, sampling_loc, attn_weight, value_dtypes=(torch.bfloat16,),
         loc_dtype=torch.float32,
