@@ -433,13 +433,11 @@ int vllm_gemm_bf16_batched(const void* A, int lda, int a_mn_major, const void* B
 int vllm_gemm_bf16_batched_grouped(const void* A, int lda, int a_mn_major, const void* B, int ldb, int b_mn_major, void* C,
                                    int ldc, int n_batch, int group, int reduce, int M, int N, int K, int causal, int out_f32,
                                    void* stream);
-/* Row kernels of the training-side path (csrc/train_ops.cu): RMSNorm backward (dx bf16, dweight fp32 ACCUMULATED --
- * zero it first), SwiGLU forward / backward on the interleaved (gate, up) columns of the gate|up GEMM, the causal
+/* Row kernels of the training-side path (csrc/train_ops.cu): RMSNorm backward (below, with vllm_rmsnorm_bwd_ws_bf16),
+ * SwiGLU forward / backward on the interleaved (gate, up) columns of the gate|up GEMM, the causal
  * softmax / softmax-backward of the materialised attention backward (in place on [n_mat*T, T] bf16 stacks), and the
  * CrossEntropyLoss of modeling_visionllmv2.py:741-757 (fp32 logits, int64 labels, -100 ignored; loss_sum accumulated,
  * dlogits bf16 = (softmax - onehot) / *n_valid). */
-int vllm_rmsnorm_bwd_bf16(const void* x, long long ldx, const void* weight, const void* dy, long long ldy, void* dx,
-                          long long lddx, float* dweight, long long rows, int cols, float eps, void* stream);
 /* Layout change of the attention backward (visionllm_b200/train.py): src [batch, tokens, parts, heads, head_dim] bf16 (parts = 3:
  * the packed q | k | v projection rows; 1: dO) -> dst [parts, batch, heads, tokens, head_dim] (every (batch, head) matrix stacked
  * along rows for vllm_gemm_bf16_batched) when to_stacked != 0, the inverse (stacked gradients -> packed d(qkv)) otherwise.
@@ -453,10 +451,9 @@ int vllm_head_stack_bf16(const void* src, void* dst, int batch, int tokens, int 
  * head_dim % 8: VLLM_EUNSUPPORTED; ld % 8 or a base not 16-byte aligned: VLLM_EALIGN. */
 int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int nq, int nkv,
                              int head_dim, int to_stacked, void* stream);
-/* The same backward with the dweight reduction done through a workspace instead of atomics: every CTA writes its partial
+/* RMSNorm backward: dx bf16 and dweight fp32, the dweight reduction done through a workspace: every CTA writes its partial
  * column sums to one row of partials [n_partials >= vllm_rmsnorm_bwd_partials(rows), cols] (fp32, 16-byte aligned) and a
- * second kernel sums the rows in order -- deterministic (the atomic form puts ~1200 atomics on each of the 4096 column
- * addresses at 8192 x 4096 rows).  dweight is overwritten (no zero-init needed). */
+ * second kernel sums the rows in order -- deterministic.  dweight is overwritten (no zero-init needed). */
 int vllm_rmsnorm_bwd_partials(long long rows);
 int vllm_rmsnorm_bwd_ws_bf16(const void* x, long long ldx, const void* weight, const void* dy, long long ldy, void* dx,
                              long long lddx, float* dweight, float* partials, int n_partials, long long rows, int cols,

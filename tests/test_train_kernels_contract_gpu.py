@@ -1,7 +1,7 @@
 """GPU: the row kernels of the training step (csrc/train_ops.cu, visionllm_b200/train.py) against float64 references of
 the same ops on the same bf16 / fp32 inputs, with exact probes, bit-identities and NaN sentinels around every output.
 
-Kernels: RMSNorm backward (partials and atomic forms), the causal softmax and its backward, SwiGLU forward / backward,
+Kernels: RMSNorm backward (per-CTA dweight partials), the causal softmax and its backward, SwiGLU forward / backward,
 the CE loss and `CrossEntropyFn`, RoPE backward (`RopeFn`, `QKVRopeFn`) and the head stacking of the attention backward.
 
 The checker is `rounds` of tests/bf16_rounding.py: away from a bf16 rounding midpoint within E of the float64 value z,
@@ -12,7 +12,7 @@ the bf16 output is RN_bf16(z) bit for bit.  u = 2^-24; no bound has a max|ref| t
                 dm = (er + (d + 3) u) mean|a n| + u |m| -- an absolute term for the cancellation in the bracket.
                 dw = sum_rows dy RN_bf16(n): where RN_bf16(n) has two candidates within (er + u)|n| the row may use either
                 (sum of |dy| |hi - lo| over those ties), plus the fp32 chain c u sum |dy| max(|lo|, |hi|) with
-                c = rows_per_cta + ceil(n_partials / 8) + 8 (partials form) or rows_per_cta + n_ctas (atomics).
+                c = rows_per_cta + ceil(n_partials / 8) + 8.
   softmax       P = softmax(s S) over keys <= query, s the fp32 scale:  E_j = 1.25 P_j (e_j + max_k e_k + (d + 3) u),
                 e_j = 2^-21 + |x_j| 2^-23 + u (|s S_j| + |max| + |x_j|), x_j = s S_j - max (__expf of an fp32 argument).
   softmax bwd   dS = s P (dP - sum P dP):  E = 1.25 s |P| (d u sum |P dP| + 3u |dP - sum P dP|).
@@ -119,15 +119,11 @@ def vpt(n_cols):
 # ---------------------------------------------------------------------------------------------------------------------
 # RMSNorm backward
 # ---------------------------------------------------------------------------------------------------------------------
-def rms_bwd(ws, x, w, dy, dx, dw, part=None, n_part=0, eps=1e-6, rows=None, cols=None):
-    L = _lib.lib()
-    rows = x.shape[0] if rows is None else rows
-    cols = x.shape[1] if cols is None else cols
-    if ws:
-        return L.vllm_rmsnorm_bwd_ws_bf16(x.data_ptr(), x.stride(0), w.data_ptr(), dy.data_ptr(), dy.stride(0), dx.data_ptr(),
-                                          dx.stride(0), dw.data_ptr(), part.data_ptr(), n_part, rows, cols, eps, stream())
-    return L.vllm_rmsnorm_bwd_bf16(x.data_ptr(), x.stride(0), w.data_ptr(), dy.data_ptr(), dy.stride(0), dx.data_ptr(),
-                                   dx.stride(0), dw.data_ptr(), rows, cols, eps, stream())
+def rms_bwd(x, w, dy, dx, dw, part, n_part, eps=1e-6):
+    rows, cols = x.shape
+    return _lib.lib().vllm_rmsnorm_bwd_ws_bf16(x.data_ptr(), x.stride(0), w.data_ptr(), dy.data_ptr(), dy.stride(0),
+                                               dx.data_ptr(), dx.stride(0), dw.data_ptr(), part.data_ptr(), n_part, rows,
+                                               cols, eps, stream())
 
 
 def rms_plan(rows):
@@ -190,10 +186,9 @@ RMS_COLS = [8, 2048, 2056, 4096, 4104, 5120, 6144, 8192]
 @pytest.mark.parametrize("kind", ["normal", "offset", "outlier", "tiny"])
 @pytest.mark.parametrize("cols", RMS_COLS)
 def test_rmsnorm_backward_vs_fp64(cols, kind):
-    """dx and dw of both forms against fp64 at 1 row, the most rows that still give one row per CTA, one more (two per
-    CTA) and 8192 rows; inputs and dy in pitched views with NaN in the gap, NaN after w, dx inside a NaN sentinel and a
-    NaN-prefilled dw.  The partials form is bit-identical across runs and pitches; dx of the atomic form is
-    bit-identical to it."""
+    """dx and dw against fp64 at 1 row, the most rows that still give one row per CTA, one more (two per CTA) and 8192
+    rows; inputs and dy in pitched views with NaN in the gap, NaN after w, dx inside a NaN sentinel and a NaN-prefilled
+    dw.  Bit-identical across runs and pitches."""
     g = gen(cols * 5 + len(kind))
     eps = 1e-6
     r1 = rows_one_per_cta()
@@ -206,7 +201,7 @@ def test_rmsnorm_backward_vs_fp64(cols, kind):
         _, gv = pitched(dy, cols + 40)
         part = torch.full((n_ctas, cols), NAN, device="cuda")
         dx, dw = Out(rows, cols, cols + 16), Out(1, cols, dtype=torch.float32)
-        assert rms_bwd(True, xv, w, gv, dx.view, dw.view[0], part, n_ctas, eps) == 0
+        assert rms_bwd(xv, w, gv, dx.view, dw.view[0], part, n_ctas, eps) == 0
         torch.cuda.synchronize()
         what = f"rows={rows} cols={cols} {kind}"
         y, yw = dx.check("dx " + what), dw.check("dw " + what)[0]
@@ -216,15 +211,8 @@ def test_rmsnorm_backward_vs_fp64(cols, kind):
         # bit-identities: a second run, contiguous views (another pitch), a larger workspace
         dx2, dw2 = torch.empty_like(x), torch.empty(cols, device="cuda")
         part2 = torch.empty((n_ctas + 3, cols), device="cuda")
-        assert rms_bwd(True, x, w, dy, dx2, dw2, part2, n_ctas + 3, eps) == 0
+        assert rms_bwd(x, w, dy, dx2, dw2, part2, n_ctas + 3, eps) == 0
         assert same_bits(dx2, y) and same_bits(dw2, yw), f"partials form not reproducible across pitches: {what}"
-        # the atomic form: the same dx, dw added to the caller's zeros within its own reorder bound
-        dxa = Out(rows, cols, cols + 8)
-        dwa = Out(1, cols, dtype=torch.float32, fill=0.0)
-        assert rms_bwd(False, xv, w, gv, dxa.view, dwa.view[0], eps=eps) == 0
-        torch.cuda.synchronize()
-        assert same_bits(dxa.check("atomic dx"), y), f"atomic dx != partials dx: {what}"
-        check_dw(dwa.check("atomic dw")[0], dy, n, En, rpc + n_ctas, "rmsnorm_bwd_dw_atomic", what)
 
 
 def test_rmsnorm_backward_probes():
@@ -238,7 +226,7 @@ def test_rmsnorm_backward_probes():
         dy = torch.zeros(rows, cols, dtype=torch.bfloat16, device="cuda")
         part = torch.full((n_ctas, cols), NAN, device="cuda")
         dx, dw = Out(rows, cols), Out(1, cols, dtype=torch.float32)
-        assert rms_bwd(True, x, w, dy, dx.view, dw.view[0], part, n_ctas) == 0
+        assert rms_bwd(x, w, dy, dx.view, dw.view[0], part, n_ctas) == 0
         torch.cuda.synchronize()
         assert (dx.check("dx") == 0).all() and (dw.check("dw") == 0).all(), f"dy = 0 is not exact 0 at cols={cols}"
 
@@ -264,8 +252,7 @@ def test_rmsnorm_backward_rejections_leave_outputs_untouched():
         "lddx % 8": (xp, lx, xp, lx, dxp, 260, 256, n_ok, EALIGN),
     }
     for what, (a, la, b, lb, c, lc, cols, npart, rc) in cases.items():
-        assert L.vllm_rmsnorm_bwd_ws_bf16(a, la, wp, b, lb, c, lc, dwp, pp, npart, 4, cols, 1e-6, st) == rc, f"ws {what}"
-        assert L.vllm_rmsnorm_bwd_bf16(a, la, wp, b, lb, c, lc, dwp, 4, cols, 1e-6, st) == rc, f"atomic {what}"
+        assert L.vllm_rmsnorm_bwd_ws_bf16(a, la, wp, b, lb, c, lc, dwp, pp, npart, 4, cols, 1e-6, st) == rc, what
     assert L.vllm_rmsnorm_bwd_ws_bf16(xp, lx, wp, xp, lx, dxp, ld, dwp, pp, n_ok - 1, 4, 256, 1e-6, st) == EINVAL
     assert L.vllm_rmsnorm_bwd_ws_bf16(xp, lx, wp, xp, lx, dxp, ld, dwp, pp + 4, n_ok, 4, 256, 1e-6, st) == EALIGN
     torch.cuda.synchronize()

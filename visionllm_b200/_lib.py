@@ -52,7 +52,6 @@ _SIGNATURES = {
     "vllm_gemm_bf16_tn": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, vp]),
     "vllm_gemm_bf16_batched": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_gemm_bf16_batched_grouped": (ci, [vp, ci, ci, vp, ci, ci, vp, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]),
-    "vllm_rmsnorm_bwd_bf16": (ci, [vp, cll, vp, vp, cll, vp, cll, vp, cll, ci, cf, vp]),
     "vllm_head_stack_bf16": (ci, [vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_head_stack_qkv_bf16": (ci, [vp, cll, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]),
     "vllm_rmsnorm_bwd_partials": (ci, [cll]),

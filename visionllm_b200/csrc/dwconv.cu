@@ -12,21 +12,9 @@
 //   y[n,h,w,c] = bias[c] + sum_{dy,dx} wt[dy*K+dx][c] * x[n, h+dy-K/2, w+dx-K/2, c]      (zeros outside the map)
 //
 // wt is the Conv2d weight [C,1,K,K] repacked tap-major [K*K][C] by the host wrapper (ops.dwconv_nhwc).
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace {
-
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-  return u;
-}
 
 template <int K, int TW>
 __global__ void __launch_bounds__(128)

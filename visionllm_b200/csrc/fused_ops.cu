@@ -12,8 +12,7 @@
 //
 // One CTA per row; 16-byte loads; the row stays in registers between the reduction and the scaling pass
 // (1 read + 1 write of the activation -- the roofline for these ops).
-#include "common.cuh"
-#include <type_traits>
+#include "rows.cuh"
 
 namespace {
 
@@ -21,48 +20,18 @@ constexpr int NT = 256;          // threads per CTA
 
 // A row is owned by TPR threads (a warp, 4 warps or the whole CTA); a CTA carries NT/TPR rows.  Each thread keeps
 // VPT 16-byte vectors of the row in registers (packed bf16) between the statistics pass and the scaling pass.
-template <int TPR>
-__device__ __forceinline__ float group_sum(float v, float* sh) {
-  v = warp_sum(v);
-  if constexpr (TPR > 32) {
-    constexpr int WPR = TPR / 32;                      // warps per row
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    const int grp = w / WPR;
-    __syncthreads();                                   // previous use of sh is over
-    if (l == 0) sh[w] = v;
-    __syncthreads();
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < WPR; ++i) t += sh[grp * WPR + i];
-    v = t;
-  }
-  return v;
-}
-
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-  return u;
-}
-
-// mode 0: RMSNorm (weight only); mode 1: LayerNorm (weight + bias)
+// mode 0: RMSNorm (weight only); mode 1: LayerNorm (weight + bias), act 1 applies exact-erf GELU to the normalised row,
+// res adds a residual row after it.
 template <int MODE, int VPT, int TPR>
 __global__ void __launch_bounds__(NT)
 norm_rows_kernel(const __nv_bfloat16* x, long long ldx, const __nv_bfloat16* __restrict__ w,
                  const __nv_bfloat16* __restrict__ b, __nv_bfloat16* y, long long ldy, long long rows,
                  int cols, float eps, int act, const __nv_bfloat16* __restrict__ res, long long ldr,
-                 const int64_t* __restrict__ gidx = nullptr, long long g_in = 0, long long g_out = 0) {
+                 const int64_t* __restrict__ gidx, long long g_in, long long g_out) {
   __shared__ float sh[NT / 32];
-  constexpr int RPC = NT / TPR;
   const int tr = threadIdx.x % TPR;
-  const long long row = (long long)blockIdx.x * RPC + threadIdx.x / TPR;
-  bool row_ok = row < rows;
+  const long long row = (long long)blockIdx.x * (NT / TPR) + threadIdx.x / TPR;
+  const bool row_ok = row < rows;
   // row gather (Swin window partition): output row (batch, j) normalises input row (batch, gidx[j]); gidx[j] >= g_in marks
   // a padded window slot -> an all-zero output row
   long long src = row;
@@ -82,40 +51,17 @@ norm_rows_kernel(const __nv_bfloat16* x, long long ldx, const __nv_bfloat16* __r
     const int v = tr + i * TPR;
     reg[i] = (v < nvec && row_ok) ? *(reinterpret_cast<const uint4*>(xr) + v) : make_uint4(0, 0, 0, 0);  // may alias y
   }
-  float s = 0.f, s2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < VPT; ++i) {
-    float f[8]; unpack8(reg[i], f);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { s += f[j]; s2 += f[j] * f[j]; }
-  }
-  float mean = 0.f, inv;
-  if (MODE == 1) {
-    mean = group_sum<TPR>(s, sh) / cols;
-    float d2 = 0.f;                                    // two-pass variance on the register-resident row
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-      if (tr + i * TPR < nvec) {
-        float f[8]; unpack8(reg[i], f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = f[j] - mean; d2 += d * d; }
-      }
-    }
-    inv = rsqrtf(group_sum<TPR>(d2, sh) / cols + eps);
-  } else {
-    inv = rsqrtf(group_sum<TPR>(s2, sh) / cols + eps);
-  }
+  float2 st;
+  if constexpr (MODE == 1) st = ln_stats<VPT, TPR, NT>(reg, cols, eps, sh);
+  else st.y = rms_rstd<VPT, TPR, true, NT>(reg, cols, eps, sh);
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int v = tr + i * TPR;
     if (v < nvec && row_ok) {
-      float f[8], wv[8], o[8];
-      unpack8(reg[i], f);
-      unpack8(__ldg(reinterpret_cast<const uint4*>(w) + v), wv);
-      if (MODE == 1) {
-        float bv[8]; unpack8(__ldg(reinterpret_cast<const uint4*>(b) + v), bv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = (f[j] - mean) * inv * wv[j] + bv[j];
+      uint4 out;
+      if constexpr (MODE == 1) {
+        float o[8];
+        ln_apply(reg[i], w, b, v, st, o);
         if (act == 1) {                                  // exact-erf GELU on the normalised row (LN -> GELU chains)
 #pragma unroll
           for (int j = 0; j < 8; ++j) o[j] = 0.5f * o[j] * (1.f + erff(o[j] * 0.70710678118654752f));
@@ -125,15 +71,11 @@ norm_rows_kernel(const __nv_bfloat16* x, long long ldx, const __nv_bfloat16* __r
 #pragma unroll
           for (int j = 0; j < 8; ++j) o[j] += rv[j];
         }
+        out = pack8(o);
       } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          // reference: (x * rsqrt).to(input_dtype) first, then weight * that (both bf16 roundings kept)
-          const float n = __bfloat162float(__float2bfloat16(f[j] * inv));
-          o[j] = wv[j] * n;
-        }
+        out = rms_apply(reg[i], w, v, st.y);
       }
-      *(reinterpret_cast<uint4*>(yr) + v) = zero_row ? make_uint4(0u, 0u, 0u, 0u) : pack8(o);
+      *(reinterpret_cast<uint4*>(yr) + v) = zero_row ? make_uint4(0u, 0u, 0u, 0u) : out;
     }
   }
 }
@@ -142,7 +84,6 @@ template <int MODE>
 int launch_norm(const void* x, long long ldx, const void* w, const void* b, void* y, long long ldy, long long rows,
                 int cols, float eps, cudaStream_t st, int act = 0, const void* res = nullptr, long long ldr = 0,
                 const int64_t* gidx = nullptr, long long g_in = 0, long long g_out = 0) {
-  const int nvec = cols / 8;
   auto go = [&](auto vpt, auto tpr) -> int {
     constexpr int VPT = decltype(vpt)::value, TPR = decltype(tpr)::value;
     const long long blocks = (rows + NT / TPR - 1) / (NT / TPR);
@@ -153,17 +94,11 @@ int launch_norm(const void* x, long long ldx, const void* w, const void* b, void
     VLLM_CHECK_LAUNCH();
     return VLLM_OK;
   };
-  using I1 = std::integral_constant<int, 1>; using I2 = std::integral_constant<int, 2>;
-  using I4 = std::integral_constant<int, 4>; using I8 = std::integral_constant<int, 8>;
-  using T32 = std::integral_constant<int, 32>; using T128 = std::integral_constant<int, 128>;
-  using T256 = std::integral_constant<int, 256>;
-  if (nvec <= 32) return go(I1{}, T32{});
-  if (nvec <= 64) return go(I2{}, T32{});
-  if (nvec <= 128) return go(I4{}, T32{});
-  if (nvec <= 256) return go(I2{}, T128{});
-  if (nvec <= 512) return go(I4{}, T128{});
-  if (nvec <= 1024) return go(I8{}, T128{});
-  return go(I8{}, T256{});
+  // a warp per row up to 128 vectors, 4 warps up to 1024, the whole CTA beyond
+  const int nvec = cols / 8;
+  if (nvec <= 128) return with_vpt<32, 1, 2, 4>(nvec, go);
+  if (nvec <= 1024) return with_vpt<128, 2, 4, 8>(nvec, go);
+  return with_vpt<256, 8>(nvec, go);
 }
 
 // qk [T, heads, 128]-style rows inside a packed tensor: element (t, h, d) at base + t*ld + h*hd + d.

@@ -8,23 +8,13 @@
 //
 // HBM-bound: 1 read for the statistics + 1 read + 1 write for the apply pass (2 B each) = 6 B / element.
 // Statistics are deterministic: per-chunk (sum, sum^2) partials in fp32, combined in double in a fixed order.
-#include "common.cuh"
+#include "rows.cuh"
 #include "vllm_b200.h"
 
 namespace {
 
 constexpr int GN_THREADS = 256;
 constexpr int GN_MAX_CHUNKS = 128;
-
-__device__ __forceinline__ void unpack8(const uint4& v, float* f) {
-  const __nv_bfloat162* p = reinterpret_cast<const __nv_bfloat162*>(&v);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __bfloat1622float2(p[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
 
 // grid (chunks, n).  Thread t owns the channel octet (t % c8) of pixels t / c8, t / c8 + ppi, ...  Octets of one
 // group are reduced through shared memory; partial[n][chunk][g] = (sum, sumsq).

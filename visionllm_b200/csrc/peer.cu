@@ -21,7 +21,7 @@
 // Memory model: writers issue plain stores to peer memory, then fence.acq_rel.sys, then red.release.sys on the
 // counter; the reader spins with ld.acquire.sys and reads the slots with ld.global.cg (L2 is the coherence point of
 // device memory written by peers; L1 is bypassed).
-#include "common.cuh"
+#include "rows.cuh"
 #include <string.h>
 
 #define TP_MAX_PEERS 8
@@ -57,18 +57,6 @@ __device__ __forceinline__ uint4 ld_cg_u4(const void* p) {
   asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
   return v;
 }
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-  return u;
-}
-
 struct TpNormArgs {
   const __nv_bfloat16* slots; int n_slots; long long slot_stride;   // [n_slots][rows][cols] partial sums (local)
   __nv_bfloat16* x;                                                  // [rows, cols] residual stream (local, in place)
@@ -95,50 +83,37 @@ tp_reduce_norm_kernel(const TpNormArgs a) {
   }
   int it = 0;
   for (int row = blockIdx.x; row < a.rows; row += gridDim.x, it ^= 1) {
-    float acc[VPT][8];
+    uint4 reg[VPT];
     __nv_bfloat16* xr = a.x + (size_t)row * a.cols;
-    float s2 = 0.f;
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int v = threadIdx.x + i * TPN_THREADS;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+      reg[i] = make_uint4(0u, 0u, 0u, 0u);
       if (v < nvec) {
+        float acc[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
         for (int s = 0; s < a.n_slots; ++s) {
           float f[8];
           unpack8(ld_cg_u4(a.slots + (size_t)s * a.slot_stride + (size_t)row * a.cols + 8 * v), f);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) acc[i][j] += f[j];
+          for (int j = 0; j < 8; ++j) acc[j] += f[j];
         }
         float f[8];
         unpack8(*(reinterpret_cast<const uint4*>(xr) + v), f);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] += f[j];
-        if (a.n_slots > 0) {
-          const uint4 pk = pack8(acc[i]);               // the new residual, rounded once to bf16 like a GEMM epilogue
-          *(reinterpret_cast<uint4*>(xr) + v) = pk;
-          unpack8(pk, acc[i]);                          // RMSNorm sees the stored (rounded) residual
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s2 += acc[i][j] * acc[i][j];
+        for (int j = 0; j < 8; ++j) acc[j] += f[j];
+        reg[i] = pack8(acc);                            // the new residual, rounded once to bf16 like a GEMM epilogue;
+        if (a.n_slots > 0) *(reinterpret_cast<uint4*>(xr) + v) = reg[i];   // RMSNorm sees the stored (rounded) value
       }
     }
-    s2 = warp_sum(s2);
-    if ((threadIdx.x & 31) == 0) sh[it][threadIdx.x >> 5] = s2;   // double-buffered: one barrier per row
-    __syncthreads();
-    float tot = 0.f;
-#pragma unroll
-    for (int i = 0; i < TPN_THREADS / 32; ++i) tot += sh[it][i];
-    const float inv = rsqrtf(tot / a.cols + a.eps);
+    // double-buffered sh: one barrier per row
+    const float inv = rms_rstd<VPT, TPN_THREADS, false>(reg, a.cols, a.eps, sh[it]);
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int v = threadIdx.x + i * TPN_THREADS;
       if (v < nvec) {
-        float wv[8], o[8];
-        unpack8(__ldg(reinterpret_cast<const uint4*>(a.w) + v), wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = wv[j] * __bfloat162float(__float2bfloat16(acc[i][j] * inv));
-        const uint4 pk = pack8(o);
+        const uint4 pk = rms_apply(reg[i], a.w, v, inv);
         for (int d = 0; d < a.n_dst; ++d)
           *(reinterpret_cast<uint4*>(a.dst[d] + (size_t)row * a.ld_dst) + v) = pk;
       }
@@ -233,13 +208,12 @@ int vllm_tp_reduce_norm_bf16(const void* slots, int n_slots, long long slot_stri
   }
   a.n_signal = n_signal; a.rows = rows; a.cols = cols;
   cudaStream_t st = (cudaStream_t)stream;
-  const int nvec = cols / 8;
   const int grid = vllm_tp_norm_ctas(rows);
-  if (nvec <= TPN_THREADS) tp_reduce_norm_kernel<1><<<grid, TPN_THREADS, 0, st>>>(a);
-  else if (nvec <= 2 * TPN_THREADS) tp_reduce_norm_kernel<2><<<grid, TPN_THREADS, 0, st>>>(a);
-  else tp_reduce_norm_kernel<4><<<grid, TPN_THREADS, 0, st>>>(a);
-  VLLM_CHECK_LAUNCH();
-  return VLLM_OK;
+  return with_vpt<TPN_THREADS, 1, 2, 4>(cols / 8, [&](auto vpt, auto) {
+    tp_reduce_norm_kernel<decltype(vpt)::value><<<grid, TPN_THREADS, 0, st>>>(a);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  });
 }
 
 int vllm_tp_wait(const void* flag, unsigned target, void* stream) {

@@ -16,8 +16,7 @@
 //                           `internvl_mlp` bridge (or a plain one-pass gather for the other bridges): output row
 //                           (n, a, b) = [x(2a, 2b) | x(2a, 2b+1) | x(2a+1, 2b) | x(2a+1, 2b+1)], x indexed (row, column) of the
 //                           tile's token grid -- the projector GEMM's A operand is produced directly.
-#include "common.cuh"
-#include <type_traits>
+#include "rows.cuh"
 
 namespace {
 
@@ -207,14 +206,9 @@ gather_rows_flat_kernel(const __nv_bfloat16* __restrict__ src, long long ld, con
   }
 }
 
-__device__ __forceinline__ void unpack8f(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-
 // One CTA (256 threads) per output row of 4*C columns; VPT 16-byte vectors per thread stay in registers between the
-// statistics and the scaling pass.  LN: with LayerNorm(4C) (weight, bias) -- same arithmetic as norm_rows_kernel<1>.
+// statistics and the scaling pass.  LN: with LayerNorm(4C) (weight, bias), the steps of norm_rows_kernel<1>.  A separate
+// kernel rather than a row source of norm_rows_kernel: folded in, its short rows (C = 96 ... 384) ran 16% slower.
 template <int VPT, bool LN>
 __global__ void __launch_bounds__(256)
 pixel_shuffle_ln_kernel(const __nv_bfloat16* __restrict__ x, long long ld_tile, long long ld_token, int skip, int gw, int gh,
@@ -228,7 +222,6 @@ pixel_shuffle_ln_kernel(const __nv_bfloat16* __restrict__ x, long long ld_tile, 
   const int cvec = C / 8, nvec = 4 * cvec;
   const __nv_bfloat16* xt = x + tile * ld_tile + (long long)skip * ld_token;
   uint4 reg[VPT];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int v = threadIdx.x + i * 256;
@@ -240,52 +233,19 @@ pixel_shuffle_ln_kernel(const __nv_bfloat16* __restrict__ x, long long ld_tile, 
       const int dy = order ? (chunk & 1) : (chunk >> 1), dx = order ? (chunk >> 1) : (chunk & 1);
       const long long tok = (long long)(2 * a + dy) * gh + (2 * b + dx);
       reg[i] = __ldg(reinterpret_cast<const uint4*>(xt + tok * ld_token) + cv);
-      if (LN) { float f[8]; unpack8f(reg[i], f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s += f[j]; }
     }
   }
-  float mean = 0.f, inv = 1.f;
-  if (LN) {
-    auto block_sum = [&](float v) {
-      v = warp_sum(v);
-      __syncthreads();
-      if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-      __syncthreads();
-      float t = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) t += sh[i];
-      return t;
-    };
-    const int cols = 4 * C;
-    mean = block_sum(s) / cols;
-    float d2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < VPT; ++i) {
-      if (threadIdx.x + i * 256 < nvec) {
-        float f[8]; unpack8f(reg[i], f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float d = f[j] - mean; d2 += d * d; }
-      }
-    }
-    inv = rsqrtf(block_sum(d2) / cols + eps);
-  }
+  float2 st;
+  if (LN) st = ln_stats<VPT, 256>(reg, 4 * C, eps, sh);
   uint4* yr = reinterpret_cast<uint4*>(y + r * 4 * C);
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int v = threadIdx.x + i * 256;
     if (v < nvec) {
       if (LN) {
-        float f[8], wv[8], bv[8], o[8];
-        unpack8f(reg[i], f);
-        unpack8f(__ldg(reinterpret_cast<const uint4*>(w) + v), wv);
-        unpack8f(__ldg(reinterpret_cast<const uint4*>(bias) + v), bv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = (f[j] - mean) * inv * wv[j] + bv[j];
-        uint4 u; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) h[j] = __floats2bfloat162_rn(o[2 * j], o[2 * j + 1]);
-        yr[v] = u;
+        float o[8];
+        ln_apply(reg[i], w, bias, v, st, o);
+        yr[v] = pack8(o);
       } else {
         yr[v] = reg[i];
       }
@@ -381,7 +341,7 @@ int vllm_pixel_shuffle_rows_bf16(const void* x, long long ld_tile, long long ld_
   const long long rows = (long long)tiles * (grid_w / 2) * (grid_h / 2);
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
   const bool ln = ln_weight != nullptr;
-  auto go = [&](auto vpt) -> int {
+  return with_vpt<256, 2, 4, 8>(nvec, [&](auto vpt, auto) -> int {
     constexpr int VPT = decltype(vpt)::value;
     if (ln)
       pixel_shuffle_ln_kernel<VPT, true><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>(
@@ -393,11 +353,7 @@ int vllm_pixel_shuffle_rows_bf16(const void* x, long long ld_tile, long long ld_
           (__nv_bfloat16*)y, chunk_order);
     VLLM_CHECK_LAUNCH();
     return VLLM_OK;
-  };
-  if (nvec <= 256 * 2) return go(std::integral_constant<int, 2>{});
-  if (nvec <= 256 * 4) return go(std::integral_constant<int, 4>{});
-  if (nvec <= 256 * 8) return go(std::integral_constant<int, 8>{});
-  return VLLM_EUNSUPPORTED;
+  });
 }
 
 }  // extern "C"

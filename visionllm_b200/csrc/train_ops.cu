@@ -11,55 +11,17 @@
 //                          the diagonal; attn_ds_kernel: dS = scale * P * (dP - sum_k dP * P)  (softmax backward), zeros above
 //   ce_loss_kernel         visionllmv2/model/modeling_visionllmv2.py:741-757: CrossEntropyLoss (mean over labels != -100) of
 //                          fp32 logits rows vs int64 labels; writes the loss sum and dlogits = (softmax - onehot) / n_valid.
-#include "common.cuh"
-#include <math.h>
-#include <type_traits>
+#include "rows.cuh"
 
 namespace {
 
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { const float2 t = __bfloat1622float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-  return u;
-}
-
-template <int NT>
-__device__ __forceinline__ float block_sum(float v, float* sh) {
-  v = warp_sum(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = 0.f;
-#pragma unroll
-  for (int i = 0; i < NT / 32; ++i) t += sh[i];
-  return t;
-}
-template <int NT>
-__device__ __forceinline__ float block_max(float v, float* sh) {
-  v = warp_max(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float t = -INFINITY;
-#pragma unroll
-  for (int i = 0; i < NT / 32; ++i) t = fmaxf(t, sh[i]);
-  return t;
-}
-
-// One CTA (256 threads) per row; VPT 16-byte vectors per thread stay in registers.  dw: fp32 [cols], atomically
-// accumulated (the caller zeroes it), one atomic per column per CTA-owned row group.
+// A CTA (256 threads) owns rows_per_cta consecutive rows; VPT 16-byte vectors per thread stay in registers.  Its dw
+// contribution (fp32, summed over its rows) goes to row blockIdx.x of partials [gridDim.x, cols].
 template <int VPT>
 __global__ void __launch_bounds__(256)
 rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __nv_bfloat16* __restrict__ w,
                    const __nv_bfloat16* __restrict__ dy, long long ldy, __nv_bfloat16* __restrict__ dx, long long lddx,
-                   float* __restrict__ dw, long long rows, int cols, float eps, int rows_per_cta,
-                   float* __restrict__ partials = nullptr) {
+                   long long rows, int cols, float eps, int rows_per_cta, float* __restrict__ partials) {
   __shared__ float sh[8];
   const int nvec = cols / 8;
   float dwacc[VPT][8];
@@ -70,7 +32,6 @@ rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __n
   const long long r0 = (long long)blockIdx.x * rows_per_cta;
   for (long long row = r0; row < r0 + rows_per_cta && row < rows; ++row) {
     uint4 xr[VPT], gr[VPT];
-    float s2 = 0.f;
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int v = threadIdx.x + i * 256;
@@ -78,12 +39,9 @@ rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __n
       if (v < nvec) {
         xr[i] = *(reinterpret_cast<const uint4*>(x + row * ldx) + v);
         gr[i] = *(reinterpret_cast<const uint4*>(dy + row * ldy) + v);
-        float f[8]; unpack8(xr[i], f);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s2 += f[j] * f[j];
       }
     }
-    const float rstd = rsqrtf(block_sum<256>(s2, sh) / cols + eps);
+    const float rstd = rms_rstd<VPT, 256>(xr, cols, eps, sh);
     float dot = 0.f;                                        // sum dn * n
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
@@ -100,7 +58,7 @@ rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __n
         }
       }
     }
-    const float mdot = block_sum<256>(dot, sh) / cols;
+    const float mdot = row_sum<256>(dot, sh) / cols;
 #pragma unroll
     for (int i = 0; i < VPT; ++i) {
       const int v = threadIdx.x + i * 256;
@@ -116,20 +74,15 @@ rmsnorm_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __n
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int v = threadIdx.x + i * 256;
-    if (v < nvec) {
-      if (partials) {                                      // one coalesced row of partials per CTA, summed by the second kernel
-        float* pr = partials + (size_t)blockIdx.x * cols + v * 8;
-        *reinterpret_cast<float4*>(pr) = make_float4(dwacc[i][0], dwacc[i][1], dwacc[i][2], dwacc[i][3]);
-        *reinterpret_cast<float4*>(pr + 4) = make_float4(dwacc[i][4], dwacc[i][5], dwacc[i][6], dwacc[i][7]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) atomicAdd(dw + v * 8 + j, dwacc[i][j]);
-      }
+    if (v < nvec) {                                        // one coalesced row of partials per CTA, summed by the second kernel
+      float* pr = partials + (size_t)blockIdx.x * cols + v * 8;
+      *reinterpret_cast<float4*>(pr) = make_float4(dwacc[i][0], dwacc[i][1], dwacc[i][2], dwacc[i][3]);
+      *reinterpret_cast<float4*>(pr + 4) = make_float4(dwacc[i][4], dwacc[i][5], dwacc[i][6], dwacc[i][7]);
     }
   }
 }
 
-// dw[c] = sum over the n per-CTA partial rows in a fixed order (deterministic, unlike the atomic form): a CTA owns 32 columns,
+// dw[c] = sum over the n per-CTA partial rows in a fixed order (deterministic): a CTA owns 32 columns,
 // its 8 warps take every 8th row (128-byte coalesced reads), shared-memory tree at the end
 __global__ void __launch_bounds__(256)
 colsum_partials_kernel(const float* __restrict__ partials, float* __restrict__ dw, int n, int cols) {
@@ -225,13 +178,13 @@ softmax_causal_kernel(__nv_bfloat16* __restrict__ s, long long lds, int T, float
       for (int j = 0; j < 8; ++j) if (vi * 8 + j <= i) { v[k][j] = f[j] * scale; mx = fmaxf(mx, v[k][j]); }
     }
   }
-  mx = block_max<256>(mx, sh);
+  mx = row_max<256>(mx, sh);
   float sum = 0.f;
 #pragma unroll
   for (int k = 0; k < VPT; ++k)
 #pragma unroll
     for (int j = 0; j < 8; ++j) { v[k][j] = __expf(v[k][j] - mx); sum += v[k][j]; }     // exp(-inf) = 0 above the diagonal
-  const float inv = 1.f / block_sum<256>(sum, sh);
+  const float inv = 1.f / row_sum<256>(sum, sh);
   // zeros are only needed inside the 256-aligned diagonal block: the causal batched GEMMs (gemm.cu, causal 2 / 3) never read
   // a 64-column k-block that lies wholly above a tile's diagonal block, and tiles are at most 256 rows
   const int wvec = min(nvec, ((i >> 8) + 1) * 32);
@@ -274,7 +227,7 @@ attn_ds_kernel(const __nv_bfloat16* __restrict__ p, __nv_bfloat16* __restrict__ 
       }
     }
   }
-  dot = block_sum<256>(dot, sh);
+  dot = row_sum<256>(dot, sh);
   const int wvec = min(nvec, ((i >> 8) + 1) * 32);            // see softmax_causal_kernel
 #pragma unroll
   for (int k = 0; k < VPT; ++k) {
@@ -353,10 +306,10 @@ ce_loss_kernel(const float* __restrict__ logits, long long ld, const int64_t* __
   }
   float mx = -INFINITY;
   for (int c = threadIdx.x; c < V; c += 512) mx = fmaxf(mx, lr[c]);
-  mx = block_max<512>(mx, sh);
+  mx = row_max<512>(mx, sh);
   float sum = 0.f;
   for (int c = threadIdx.x; c < V; c += 512) sum += expf(lr[c] - mx);
-  sum = block_sum<512>(sum, sh);
+  sum = row_sum<512>(sum, sh);
   const float lse = mx + logf(sum);
   if (threadIdx.x == 0) atomicAdd(loss_sum, lse - lr[label]);
   if (dr) {
@@ -390,30 +343,6 @@ scale_rows_kernel(__nv_bfloat16* __restrict__ x, long long ld, int cols, const f
 
 extern "C" {
 
-int vllm_rmsnorm_bwd_bf16(const void* x, long long ldx, const void* weight, const void* dy, long long ldy, void* dx,
-                          long long lddx, float* dweight, long long rows, int cols, float eps, void* stream) {
-  if (rows < 0 || cols <= 0 || cols % 8) return VLLM_EINVAL;
-  if (rows == 0) return VLLM_OK;
-  if (!x || !weight || !dy || !dx || !dweight) return VLLM_EINVAL;
-  if (ldx % 8 || ldy % 8 || lddx % 8 || !vllm_aligned(x, 16) || !vllm_aligned(dy, 16) || !vllm_aligned(dx, 16)) return VLLM_EALIGN;
-  const int nvec = cols / 8;
-  const int rows_per_cta = (int)((rows + (long long)vllm_num_sms() * 8 - 1) / ((long long)vllm_num_sms() * 8));
-  const long long blocks = (rows + rows_per_cta - 1) / rows_per_cta;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto vpt) -> int {
-    constexpr int VPT = decltype(vpt)::value;
-    rmsnorm_bwd_kernel<VPT><<<(unsigned)blocks, 256, 0, st>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight,
-                                                             (const __nv_bfloat16*)dy, ldy, (__nv_bfloat16*)dx, lddx, dweight,
-                                                             rows, cols, eps, rows_per_cta);
-    VLLM_CHECK_LAUNCH();
-    return VLLM_OK;
-  };
-  if (nvec <= 256) return go(std::integral_constant<int, 1>{});
-  if (nvec <= 512) return go(std::integral_constant<int, 2>{});
-  if (nvec <= 1024) return go(std::integral_constant<int, 4>{});
-  return VLLM_EUNSUPPORTED;
-}
-
 static int rmsnorm_bwd_ctas(long long rows) {
   const int rows_per_cta = (int)((rows + (long long)vllm_num_sms() * 8 - 1) / ((long long)vllm_num_sms() * 8));
   return rows_per_cta > 0 ? (int)((rows + rows_per_cta - 1) / rows_per_cta) : 0;
@@ -431,25 +360,19 @@ int vllm_rmsnorm_bwd_ws_bf16(const void* x, long long ldx, const void* weight, c
   if (ldx % 8 || ldy % 8 || lddx % 8 || !vllm_aligned(x, 16) || !vllm_aligned(dy, 16) || !vllm_aligned(dx, 16) ||
       !vllm_aligned(partials, 16))
     return VLLM_EALIGN;
-  const int nvec = cols / 8;
   const int rows_per_cta = (int)((rows + (long long)vllm_num_sms() * 8 - 1) / ((long long)vllm_num_sms() * 8));
   const int blocks = rmsnorm_bwd_ctas(rows);
   if (n_partials < blocks) return VLLM_EINVAL;
   cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto vpt) -> int {
-    constexpr int VPT = decltype(vpt)::value;
-    rmsnorm_bwd_kernel<VPT><<<(unsigned)blocks, 256, 0, st>>>((const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight,
-                                                             (const __nv_bfloat16*)dy, ldy, (__nv_bfloat16*)dx, lddx, dweight,
-                                                             rows, cols, eps, rows_per_cta, partials);
+  return with_vpt<256, 1, 2, 4>(cols / 8, [&](auto vpt, auto) {
+    rmsnorm_bwd_kernel<decltype(vpt)::value><<<(unsigned)blocks, 256, 0, st>>>(
+        (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, (const __nv_bfloat16*)dy, ldy, (__nv_bfloat16*)dx, lddx,
+        rows, cols, eps, rows_per_cta, partials);
     VLLM_CHECK_LAUNCH();
     colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials, dweight, blocks, cols);
     VLLM_CHECK_LAUNCH();
     return VLLM_OK;
-  };
-  if (nvec <= 256) return go(std::integral_constant<int, 1>{});
-  if (nvec <= 512) return go(std::integral_constant<int, 2>{});
-  if (nvec <= 1024) return go(std::integral_constant<int, 4>{});
-  return VLLM_EUNSUPPORTED;
+  });
 }
 
 int vllm_head_stack_bf16(const void* src, void* dst, int batch, int tokens, int parts, int heads, int head_dim,
@@ -527,14 +450,11 @@ int vllm_softmax_causal_bf16(void* s, long long ld, long long n_mat, int T, floa
   if (!vllm_aligned(s, 16)) return VLLM_EALIGN;
   const long long rows = n_mat * T;
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nvec = T / 8;
-  if (nvec <= 256) softmax_causal_kernel<1><<<(unsigned)rows, 256, 0, st>>>((__nv_bfloat16*)s, ld, T, scale);
-  else if (nvec <= 512) softmax_causal_kernel<2><<<(unsigned)rows, 256, 0, st>>>((__nv_bfloat16*)s, ld, T, scale);
-  else if (nvec <= 1024) softmax_causal_kernel<4><<<(unsigned)rows, 256, 0, st>>>((__nv_bfloat16*)s, ld, T, scale);
-  else return VLLM_EUNSUPPORTED;
-  VLLM_CHECK_LAUNCH();
-  return VLLM_OK;
+  return with_vpt<256, 1, 2, 4>(T / 8, [&](auto vpt, auto) {
+    softmax_causal_kernel<decltype(vpt)::value><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)s, ld, T, scale);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  });
 }
 
 int vllm_attn_ds_bf16(const void* p, void* dp, long long ld, long long n_mat, int T, float scale, void* stream) {
@@ -544,14 +464,12 @@ int vllm_attn_ds_bf16(const void* p, void* dp, long long ld, long long n_mat, in
   if (!vllm_aligned(p, 16) || !vllm_aligned(dp, 16)) return VLLM_EALIGN;
   const long long rows = n_mat * T;
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nvec = T / 8;
-  if (nvec <= 256) attn_ds_kernel<1><<<(unsigned)rows, 256, 0, st>>>((const __nv_bfloat16*)p, (__nv_bfloat16*)dp, ld, T, scale);
-  else if (nvec <= 512) attn_ds_kernel<2><<<(unsigned)rows, 256, 0, st>>>((const __nv_bfloat16*)p, (__nv_bfloat16*)dp, ld, T, scale);
-  else if (nvec <= 1024) attn_ds_kernel<4><<<(unsigned)rows, 256, 0, st>>>((const __nv_bfloat16*)p, (__nv_bfloat16*)dp, ld, T, scale);
-  else return VLLM_EUNSUPPORTED;
-  VLLM_CHECK_LAUNCH();
-  return VLLM_OK;
+  return with_vpt<256, 1, 2, 4>(T / 8, [&](auto vpt, auto) {
+    attn_ds_kernel<decltype(vpt)::value><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)p,
+                                                                                         (__nv_bfloat16*)dp, ld, T, scale);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  });
 }
 
 int vllm_ce_loss_f32(const float* logits, long long ld, const int64_t* labels, const int64_t* n_valid, long long rows, int vocab,

@@ -34,14 +34,6 @@ from . import _lib, ops
 from .llama import rope_tables
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _check(rc, what):
-    _lib.check(rc, what)
-
-
 # ---- thin wrappers over the C-ABI row kernels ------------------------------------------------------------------------
 def rmsnorm_bwd(x2, weight, dy2, eps):
     rows, cols = x2.shape
@@ -53,8 +45,8 @@ def rmsnorm_bwd(x2, weight, dy2, eps):
     with torch.cuda.device(x2.device):
         rc = L.vllm_rmsnorm_bwd_ws_bf16(x2.data_ptr(), x2.stride(0), weight.data_ptr(), dy2.data_ptr(), dy2.stride(0),
                                         dx.data_ptr(), dx.stride(0), dw.data_ptr(), part.data_ptr(), n_part, rows, cols,
-                                        float(eps), _stream())
-    _check(rc, "vllm_rmsnorm_bwd_ws_bf16")
+                                        float(eps), ops._stream())
+    _lib.check(rc, "vllm_rmsnorm_bwd_ws_bf16")
     return dx, dw
 
 
@@ -62,8 +54,8 @@ def swiglu_fwd(gu):
     rows, two_i = gu.shape
     h = torch.empty((rows, two_i // 2), dtype=gu.dtype, device=gu.device)
     with torch.cuda.device(gu.device):
-        rc = _lib.lib().vllm_swiglu_fwd_bf16(gu.data_ptr(), gu.stride(0), h.data_ptr(), h.stride(0), rows, two_i // 2, _stream())
-    _check(rc, "vllm_swiglu_fwd_bf16")
+        rc = _lib.lib().vllm_swiglu_fwd_bf16(gu.data_ptr(), gu.stride(0), h.data_ptr(), h.stride(0), rows, two_i // 2, ops._stream())
+    _lib.check(rc, "vllm_swiglu_fwd_bf16")
     return h
 
 
@@ -72,8 +64,8 @@ def swiglu_bwd(gu, dh):
     dgu = torch.empty_like(gu)
     with torch.cuda.device(gu.device):
         rc = _lib.lib().vllm_swiglu_bwd_bf16(gu.data_ptr(), gu.stride(0), dh.data_ptr(), dh.stride(0), dgu.data_ptr(),
-                                             dgu.stride(0), rows, two_i // 2, _stream())
-    _check(rc, "vllm_swiglu_bwd_bf16")
+                                             dgu.stride(0), rows, two_i // 2, ops._stream())
+    _lib.check(rc, "vllm_swiglu_bwd_bf16")
     return dgu
 
 
@@ -82,8 +74,8 @@ def head_stack(t, B, T, parts, H, D, to_stacked):
     src = t if t.is_contiguous() else t.contiguous()
     out = torch.empty((parts, B, H, T, D) if to_stacked else (B, T, parts, H, D), dtype=src.dtype, device=src.device)
     with torch.cuda.device(src.device):
-        rc = _lib.lib().vllm_head_stack_bf16(src.data_ptr(), out.data_ptr(), B, T, parts, H, D, 1 if to_stacked else 0, _stream())
-    _check(rc, "vllm_head_stack_bf16")
+        rc = _lib.lib().vllm_head_stack_bf16(src.data_ptr(), out.data_ptr(), B, T, parts, H, D, 1 if to_stacked else 0, ops._stream())
+    _lib.check(rc, "vllm_head_stack_bf16")
     return out
 
 
@@ -99,8 +91,8 @@ def head_stack_qkv(qkv, nq, nkv, D, stacks=None):
     q, k, v = stacks[:nq_rows], stacks[nq_rows:nq_rows + nkv_rows], stacks[nq_rows + nkv_rows:]
     with torch.cuda.device(qkv.device):
         rc = _lib.lib().vllm_head_stack_qkv_bf16(qkv.data_ptr(), qkv.stride(1), q.data_ptr(), k.data_ptr(), v.data_ptr(), B, T,
-                                                 nq, nkv, D, 1 if to_stacked else 0, _stream())
-    _check(rc, "vllm_head_stack_qkv_bf16")
+                                                 nq, nkv, D, 1 if to_stacked else 0, ops._stream())
+    _lib.check(rc, "vllm_head_stack_qkv_bf16")
     return stacks if to_stacked else qkv
 
 
@@ -115,8 +107,8 @@ def gemm_batched(a, b, n_batch, M, N, K, a_mn=False, b_mn=False, causal=0, out_d
                                                f"b{n_batch}x{M}x{N}x{K}" + (f"g{group}{'r' if reduce else ''}" if group > 1 else "")):
         rc = _lib.lib().vllm_gemm_bf16_batched_grouped(a.data_ptr(), a.stride(0), int(a_mn), b.data_ptr(), b.stride(0), int(b_mn),
                                                        out.data_ptr(), out.stride(0), n_batch, group, int(reduce), M, N, K,
-                                                       int(causal), 1 if out_dtype == torch.float32 else 0, _stream())
-    _check(rc, "vllm_gemm_bf16_batched_grouped")
+                                                       int(causal), 1 if out_dtype == torch.float32 else 0, ops._stream())
+    _lib.check(rc, "vllm_gemm_bf16_batched_grouped")
     return out
 
 
@@ -143,10 +135,10 @@ def attention_backward_packed(qkv5, do, scale):
     L_ = _lib.lib()
     p = gemm_batched(qs, ks, BQ, T, T, D, causal=1, group=G)                     # S = Q K^T, tiles above the diagonal skipped
     with torch.cuda.device(qkv5.device):
-        _check(L_.vllm_softmax_causal_bf16(p.data_ptr(), p.stride(0), BQ, T, float(scale), _stream()), "vllm_softmax_causal_bf16")
+        _lib.check(L_.vllm_softmax_causal_bf16(p.data_ptr(), p.stride(0), BQ, T, float(scale), ops._stream()), "vllm_softmax_causal_bf16")
     dp = gemm_batched(dos, vs, BQ, T, T, D, causal=1, group=G)                   # dP = dO V^T
     with torch.cuda.device(qkv5.device):
-        _check(L_.vllm_attn_ds_bf16(p.data_ptr(), dp.data_ptr(), p.stride(0), BQ, T, float(scale), _stream()), "vllm_attn_ds_bf16")
+        _lib.check(L_.vllm_attn_ds_bf16(p.data_ptr(), dp.data_ptr(), p.stride(0), BQ, T, float(scale), ops._stream()), "vllm_attn_ds_bf16")
     ds = dp
     dstk = torch.empty_like(stk)
     dqs, dks, dvs = dstk[:BQ * T], dstk[BQ * T:(BQ + BKV) * T], dstk[(BQ + BKV) * T:]
@@ -322,8 +314,8 @@ class CrossEntropyFn(torch.autograd.Function):
         dlogits = torch.empty((rows, (V + 7) // 8 * 8), dtype=torch.bfloat16, device=logits.device)[:, :V]
         with torch.cuda.device(logits.device):
             rc = _lib.lib().vllm_ce_loss_f32(logits.data_ptr(), logits.stride(0), labels.data_ptr(), n_valid.data_ptr(), rows, V,
-                                             loss_sum.data_ptr(), dlogits.data_ptr(), dlogits.stride(0), _stream())
-        _check(rc, "vllm_ce_loss_f32")
+                                             loss_sum.data_ptr(), dlogits.data_ptr(), dlogits.stride(0), ops._stream())
+        _lib.check(rc, "vllm_ce_loss_f32")
         ctx.save_for_backward(dlogits)
         return (loss_sum / n_valid.clamp(min=1).float()).reshape(())
 
@@ -335,8 +327,8 @@ class CrossEntropyFn(torch.autograd.Function):
         scale = dloss.detach().to(torch.float32).reshape(1).contiguous()
         rows, V = dlogits.shape
         with torch.cuda.device(dlogits.device):
-            rc = _lib.lib().vllm_scale_rows_bf16(dlogits.data_ptr(), dlogits.stride(0), rows, V, scale.data_ptr(), _stream())
-        _check(rc, "vllm_scale_rows_bf16")
+            rc = _lib.lib().vllm_scale_rows_bf16(dlogits.data_ptr(), dlogits.stride(0), rows, V, scale.data_ptr(), ops._stream())
+        _lib.check(rc, "vllm_scale_rows_bf16")
         return dlogits, None
 
 
