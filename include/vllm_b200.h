@@ -469,6 +469,40 @@ int vllm_ce_loss_f32(const float* logits, long long ld, const int64_t* labels, c
  * device (the upstream gradient of the loss: CrossEntropyFn.backward scales dlogits by it without a host sync).
  * ld % 8 or a base not 16-byte aligned: VLLM_EALIGN. */
 int vllm_scale_rows_bf16(void* x, long long ld, long long rows, int cols, const float* scale, void* stream);
+/* Attention backward on right-padded batches of any length (visionllm_b200/train.py): the stacks are padded to tokens_pad
+ * rows per (batch, head) matrix (a multiple of 256 for the batched GEMMs).  vllm_head_stack_qkv_pad_bf16 is
+ * vllm_head_stack_qkv_bf16 with stacks of tokens_pad rows: rows tokens .. tokens_pad - 1 are written as zeros going to the
+ * stacks and are not read coming back; nkv = 0 stacks the nq heads of a plain [batch, tokens, nq head_dim] tensor (dO) into q.
+ * vllm_softmax_causal_len_bf16 is vllm_softmax_causal_bf16 with key lengths lens[n_mat / heads_per_batch] (int32, device):
+ * key j of query i is visible iff j <= i and j < lens[m / heads_per_batch]; P = 0 elsewhere (S is not used there), a row
+ * with no visible key is all zeros.  n_mat % heads_per_batch: VLLM_EINVAL.  With lens == T it is bit-identical to
+ * vllm_softmax_causal_bf16. */
+int vllm_head_stack_qkv_pad_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int tokens_pad,
+                                 int nq, int nkv, int head_dim, int to_stacked, void* stream);
+int vllm_softmax_causal_len_bf16(void* s, long long ld, long long n_mat, int heads_per_batch, int T, const int* lens,
+                                 float scale, void* stream);
+/* Backward of the vision-language bridge.  Every parameter gradient is fp32, summed over rows in a fixed order (per-CTA
+ * partials in row order, then the partial rows in order, as vllm_rmsnorm_bwd_ws_bf16): run-to-run identical.
+ *   vllm_gelu_fwd_bf16   y = gelu(u), exact erf (nn.GELU()), [rows, cols] bf16;
+ *   vllm_gelu_bwd_bf16   dx = dy * gelu'(u) from the saved pre-activation u;
+ *   vllm_bias_grad_bf16  dbias[c] = sum over rows of dy[r, c];
+ *   vllm_layernorm_bwd_wb_bf16  nn.LayerNorm weight / bias gradients, dweight = sum dy * (x - mean) * rstd, dbias = sum dy
+ *                        (no dx).  partials [2 n_partials, cols].
+ * partials: fp32, 16-byte aligned, n_partials >= vllm_rmsnorm_bwd_partials(rows) rows of cols.  cols % 8: VLLM_EINVAL. */
+int vllm_gelu_fwd_bf16(const void* u, long long ldu, void* y, long long ldy, long long rows, int cols, void* stream);
+int vllm_gelu_bwd_bf16(const void* u, long long ldu, const void* dy, long long lddy, void* dx, long long lddx, long long rows,
+                       int cols, void* stream);
+int vllm_bias_grad_bf16(const void* dy, long long ldy, float* dbias, float* partials, int n_partials, long long rows, int cols,
+                        void* stream);
+int vllm_layernorm_bwd_wb_bf16(const void* x, long long ldx, const void* dy, long long ldy, float* dweight, float* dbias,
+                               float* partials, int n_partials, long long rows, int cols, float eps, void* stream);
+/* Backward of vllm_assemble_embeds_bf16: the n positions sorted stably by destination row (dest ascending, int32; order[s] the
+ * position of entry s) -> d_sources [source_rows, hidden] bf16, every row the fp32 sum, in position order, of the d_embeds
+ * rows of the positions naming it, rounded once; rows no position names are exact 0.  The destinations index the
+ * concatenation of the sources (token table | [EMB] det table | [EMB] pose table | image features), so one call gives the
+ * table gradients and the gather of d(image features) (each feature row is named at most once: an exact copy). */
+int vllm_assemble_embeds_bwd_bf16(const int* dest, const int* order, long long n, const void* d_embeds, int hidden,
+                                  void* d_sources, long long source_rows, void* stream);
 
 /* ---- sequence assembly of VisionLLMv2Model.forward (SURVEY 8f rank 2, 8a-a7/a9; csrc/seqglue.cu) -----------------
  * vllm_seq_index: ONE pass over input_ids [batch, seq_len] (int64, device) producing

@@ -62,6 +62,13 @@ _SIGNATURES = {
     "vllm_attn_ds_bf16": (ci, [vp, vp, cll, cll, ci, cf, vp]),
     "vllm_ce_loss_f32": (ci, [vp, cll, vp, vp, cll, ci, vp, vp, cll, vp]),
     "vllm_scale_rows_bf16": (ci, [vp, cll, cll, ci, vp, vp]),
+    "vllm_head_stack_qkv_pad_bf16": (ci, [vp, cll, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp]),
+    "vllm_softmax_causal_len_bf16": (ci, [vp, cll, cll, ci, ci, vp, cf, vp]),
+    "vllm_gelu_fwd_bf16": (ci, [vp, cll, vp, cll, cll, ci, vp]),
+    "vllm_gelu_bwd_bf16": (ci, [vp, cll, vp, cll, vp, cll, cll, ci, vp]),
+    "vllm_bias_grad_bf16": (ci, [vp, cll, vp, vp, ci, cll, ci, vp]),
+    "vllm_layernorm_bwd_wb_bf16": (ci, [vp, cll, vp, cll, vp, vp, vp, ci, cll, ci, cf, vp]),
+    "vllm_assemble_embeds_bwd_bf16": (ci, [vp, vp, cll, vp, ci, vp, cll, vp]),
     "vllm_gemm_set_variant": (ci, [ci]),
     "vllm_rmsnorm_bf16": (ci, [vp, cll, vp, vp, cll, cll, ci, cf, vp]),
     "vllm_layernorm_bf16": (ci, [vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),

@@ -156,13 +156,17 @@ swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ gu, long long ldgu, const __
 }
 
 // S [n_mat, T, T] bf16 (row pitch lds, matrix pitch T*lds) -> P in place: softmax over keys j <= i of scale * S, zeros for j > i.
+// With `lens` (key lengths, one per batch row of heads_per_batch consecutive matrices) the keys are j <= i and j < len:
+// P = 0 for j >= len, and S is not used there (a NaN in a masked key cannot leak); a row with no key is all zeros.
 // One CTA per row; T <= 256 * 8 * VPT.
 template <int VPT>
 __global__ void __launch_bounds__(256)
-softmax_causal_kernel(__nv_bfloat16* __restrict__ s, long long lds, int T, float scale) {
+softmax_causal_kernel(__nv_bfloat16* __restrict__ s, long long lds, int T, float scale, const int* __restrict__ lens,
+                      int heads_per_batch) {
   __shared__ float sh[8];
   const long long row_g = blockIdx.x;                        // matrix * T + i
   const int i = (int)(row_g % T);
+  const int last = lens ? min(i, lens[row_g / T / heads_per_batch] - 1) : i;   // last visible key
   __nv_bfloat16* sr = s + row_g * lds;
   const int nvec = T / 8;
   float v[VPT][8];
@@ -172,19 +176,21 @@ softmax_causal_kernel(__nv_bfloat16* __restrict__ s, long long lds, int T, float
     const int vi = threadIdx.x + k * 256;
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[k][j] = -INFINITY;
-    if (vi < nvec && vi * 8 <= i) {
+    if (vi < nvec && vi * 8 <= last) {
       float f[8]; unpack8(*(reinterpret_cast<const uint4*>(sr) + vi), f);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) if (vi * 8 + j <= i) { v[k][j] = f[j] * scale; mx = fmaxf(mx, v[k][j]); }
+      for (int j = 0; j < 8; ++j) if (vi * 8 + j <= last) { v[k][j] = f[j] * scale; mx = fmaxf(mx, v[k][j]); }
     }
   }
   mx = row_max<256>(mx, sh);
+  if (lens && mx == -INFINITY) mx = 0.f;                     // no visible key (length 0): exp(-inf) = 0 everywhere
   float sum = 0.f;
 #pragma unroll
   for (int k = 0; k < VPT; ++k)
 #pragma unroll
     for (int j = 0; j < 8; ++j) { v[k][j] = __expf(v[k][j] - mx); sum += v[k][j]; }     // exp(-inf) = 0 above the diagonal
-  const float inv = 1.f / row_sum<256>(sum, sh);
+  sum = row_sum<256>(sum, sh);
+  const float inv = lens && !(sum > 0.f) ? 0.f : 1.f / sum;  // without lengths: the original arithmetic for any input
   // zeros are only needed inside the 256-aligned diagonal block: the causal batched GEMMs (gemm.cu, causal 2 / 3) never read
   // a 64-column k-block that lies wholly above a tile's diagonal block, and tiles are at most 256 rows
   const int wvec = min(nvec, ((i >> 8) + 1) * 32);
@@ -262,13 +268,14 @@ head_stack_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int B,
 }
 
 // Grouped-query form of the same layout change: packed projection rows [B, T, (nq + 2 nkv) D] with row pitch ld_vec
-// 16-byte vectors (q heads, then k heads, then v heads) <-> three stacks Q [B, nq, T, D], K [B, nkv, T, D], V [B, nkv, T, D].
+// 16-byte vectors (q heads, then k heads, then v heads) <-> three stacks Q [B, nq, TP, D], K [B, nkv, TP, D], V [B, nkv, TP, D].
 // i indexes the concatenation Q | K | V of the stacks (coalesced on the stacked side); the pitch gap of a packed row is
-// neither read nor written.
+// neither read nor written.  Stack rows t >= T (TP > T pads every matrix) are written as zeros going to the stacks and
+// skipped coming back.  NKV = 0 stacks the q heads alone.
 __global__ void __launch_bounds__(256)
 head_stack_qkv_kernel(uint4* __restrict__ packed, long long ld_vec, uint4* __restrict__ q, uint4* __restrict__ k,
-                      uint4* __restrict__ v, int B, int T, int NQ, int NKV, int DV, int to_stacked, long long n_vec) {
-  const long long n_q = (long long)B * NQ * T * DV, n_kv = (long long)B * NKV * T * DV;
+                      uint4* __restrict__ v, int B, int T, int TP, int NQ, int NKV, int DV, int to_stacked, long long n_vec) {
+  const long long n_q = (long long)B * NQ * TP * DV, n_kv = (long long)B * NKV * TP * DV;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_vec; i += (long long)gridDim.x * blockDim.x) {
     long long r = i;
     uint4* st = q; int heads = NQ, h0 = 0;
@@ -279,9 +286,13 @@ head_stack_qkv_kernel(uint4* __restrict__ packed, long long ld_vec, uint4* __res
     }
     const long long si = r;
     const int d = (int)(r % DV); r /= DV;
-    const int t = (int)(r % T); r /= T;
+    const int t = (int)(r % TP); r /= TP;
     const int h = (int)(r % heads);
     const int b = (int)(r / heads);
+    if (t >= T) {
+      if (to_stacked) st[si] = make_uint4(0u, 0u, 0u, 0u);
+      continue;
+    }
     const long long pi = ((long long)b * T + t) * ld_vec + (long long)(h0 + h) * DV + d;
     if (to_stacked) st[si] = packed[pi];
     else packed[pi] = st[si];
@@ -337,6 +348,133 @@ scale_rows_kernel(__nv_bfloat16* __restrict__ x, long long ld, int cols, const f
     *p = pack8(f);
   }
   for (int c = nvec * 8 + threadIdx.x; c < cols; c += 256) xr[c] = __float2bfloat16(__bfloat162float(xr[c]) * s);
+}
+
+// ---- backward of the vision-language bridge and of the sequence assembly (the multimodal training step) ----
+
+__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
+// d/du of 0.5 u (1 + erf(u / sqrt 2)) = Phi(u) + u phi(u)
+__device__ __forceinline__ float gelu_erf_grad(float u) {
+  return 0.5f * (1.f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * expf(-0.5f * u * u);
+}
+
+// y = gelu(u) (BACKWARD = 0) or dx = dy * gelu'(u) (BACKWARD = 1) on [rows, cols] bf16, 8 elements per thread
+template <bool BACKWARD>
+__global__ void __launch_bounds__(256)
+gelu_kernel(const __nv_bfloat16* __restrict__ u, long long ldu, const __nv_bfloat16* __restrict__ dy, long long lddy,
+            __nv_bfloat16* __restrict__ out, long long ldo, long long rows, int cols) {
+  const int vec_per_row = cols / 8;
+  const long long total = rows * vec_per_row;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / vec_per_row;
+    const int v = (int)(i - row * vec_per_row);
+    float a[8], o[8];
+    unpack8(*(reinterpret_cast<const uint4*>(u + row * ldu) + v), a);
+    if constexpr (BACKWARD) {
+      float g[8];
+      unpack8(*(reinterpret_cast<const uint4*>(dy + row * lddy) + v), g);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = g[j] * gelu_erf_grad(a[j]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = gelu_erf(a[j]);
+    }
+    *(reinterpret_cast<uint4*>(out + row * ldo) + v) = pack8(o);
+  }
+}
+
+// Column sums of dy [rows, cols] over the rows of a CTA, in row order: CTA (x, y) owns rows [x rpc, (x + 1) rpc) and the
+// 256 16-byte column vectors of block y; its sums go to row x of partials [gridDim.x, cols] (then colsum_partials_kernel).
+__global__ void __launch_bounds__(256)
+colsum_rows_kernel(const __nv_bfloat16* __restrict__ dy, long long ldy, long long rows, int cols, int rows_per_cta,
+                   float* __restrict__ partials) {
+  const int v = blockIdx.y * 256 + threadIdx.x;
+  if (v >= cols / 8) return;
+  float acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+  const long long r0 = (long long)blockIdx.x * rows_per_cta;
+  for (long long row = r0; row < r0 + rows_per_cta && row < rows; ++row) {
+    float g[8];
+    unpack8(*(reinterpret_cast<const uint4*>(dy + row * ldy) + v), g);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] += g[j];
+  }
+  float* pr = partials + (size_t)blockIdx.x * cols + v * 8;
+  *reinterpret_cast<float4*>(pr) = make_float4(acc[0], acc[1], acc[2], acc[3]);
+  *reinterpret_cast<float4*>(pr + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// nn.LayerNorm weight / bias gradients: xhat = (x - mean) * rstd (fp32, the forward's statistics recomputed by ln_stats);
+// dgamma += dy * xhat, dbeta += dy over the CTA's rows in order -> rows x (dgamma) and n + x (dbeta) of partials [2n, cols].
+template <int VPT>
+__global__ void __launch_bounds__(256)
+layernorm_bwd_wb_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __nv_bfloat16* __restrict__ dy,
+                        long long ldy, long long rows, int cols, float eps, int rows_per_cta, float* __restrict__ partials) {
+  __shared__ float sh[8];
+  const int nvec = cols / 8;
+  float gacc[VPT][8], bacc[VPT][8];
+#pragma unroll
+  for (int i = 0; i < VPT; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) gacc[i][j] = bacc[i][j] = 0.f;
+  const long long r0 = (long long)blockIdx.x * rows_per_cta;
+  for (long long row = r0; row < r0 + rows_per_cta && row < rows; ++row) {
+    uint4 xr[VPT];
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int v = threadIdx.x + i * 256;
+      xr[i] = v < nvec ? *(reinterpret_cast<const uint4*>(x + row * ldx) + v) : make_uint4(0u, 0u, 0u, 0u);
+    }
+    const float2 st = ln_stats<VPT, 256>(xr, cols, eps, sh);
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int v = threadIdx.x + i * 256;
+      if (v < nvec) {
+        float f[8], g[8];
+        unpack8(xr[i], f); unpack8(*(reinterpret_cast<const uint4*>(dy + row * ldy) + v), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { gacc[i][j] += g[j] * ((f[j] - st.x) * st.y); bacc[i][j] += g[j]; }
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < VPT; ++i) {
+    const int v = threadIdx.x + i * 256;
+    if (v < nvec) {
+      float* pg = partials + (size_t)blockIdx.x * cols + v * 8;
+      float* pb = partials + (size_t)(gridDim.x + blockIdx.x) * cols + v * 8;
+      *reinterpret_cast<float4*>(pg) = make_float4(gacc[i][0], gacc[i][1], gacc[i][2], gacc[i][3]);
+      *reinterpret_cast<float4*>(pg + 4) = make_float4(gacc[i][4], gacc[i][5], gacc[i][6], gacc[i][7]);
+      *reinterpret_cast<float4*>(pb) = make_float4(bacc[i][0], bacc[i][1], bacc[i][2], bacc[i][3]);
+      *reinterpret_cast<float4*>(pb + 4) = make_float4(bacc[i][4], bacc[i][5], bacc[i][6], bacc[i][7]);
+    }
+  }
+}
+
+// Segment sums of the assembly backward: positions sorted stably by destination row (dest[s], ascending, with order[s] the
+// position) -> every row r < n_rows of d_src = sum over the positions with destination r of dy[position], fp32 in
+// position order, one bf16 rounding; a row no position names is exact 0.  One CTA per destination row.
+__global__ void __launch_bounds__(256)
+segment_sum_rows_kernel(const int* __restrict__ dest, const int* __restrict__ order, long long n,
+                        const __nv_bfloat16* __restrict__ dy, int C, __nv_bfloat16* __restrict__ out, long long n_rows) {
+  const int nvec = C / 8;
+  for (long long r = blockIdx.x; r < n_rows; r += gridDim.x) {
+    long long lo = 0, hi = n;                                 // first s with dest[s] >= r
+    while (lo < hi) { const long long mid = (lo + hi) >> 1; if (dest[mid] < r) lo = mid + 1; else hi = mid; }
+    for (int v = threadIdx.x; v < nvec; v += 256) {
+      float acc[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+      for (long long s = lo; s < n && dest[s] == r; ++s) {
+        float g[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(dy + (long long)order[s] * C) + v), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] += g[j];
+      }
+      *(reinterpret_cast<uint4*>(out + r * C) + v) = pack8(acc);
+    }
+  }
 }
 
 }  // namespace
@@ -406,7 +544,7 @@ int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void*
   const long long cap = (long long)vllm_num_sms() * 16;
   if (blocks > cap) blocks = cap;
   head_stack_qkv_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((uint4*)packed, ld / 8, (uint4*)q, (uint4*)k,
-                                                                           (uint4*)v, batch, tokens, nq, nkv, head_dim / 8,
+                                                                           (uint4*)v, batch, tokens, tokens, nq, nkv, head_dim / 8,
                                                                            to_stacked ? 1 : 0, n_vec);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
@@ -451,7 +589,8 @@ int vllm_softmax_causal_bf16(void* s, long long ld, long long n_mat, int T, floa
   const long long rows = n_mat * T;
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
   return with_vpt<256, 1, 2, 4>(T / 8, [&](auto vpt, auto) {
-    softmax_causal_kernel<decltype(vpt)::value><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)s, ld, T, scale);
+    softmax_causal_kernel<decltype(vpt)::value><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)s, ld, T, scale,
+                                                                                                nullptr, 1);
     VLLM_CHECK_LAUNCH();
     return VLLM_OK;
   });
@@ -491,6 +630,135 @@ int vllm_scale_rows_bf16(void* x, long long ld, long long rows, int cols, const 
   if (ld % 8 || !vllm_aligned(x, 16)) return VLLM_EALIGN;
   if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
   scale_rows_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)x, ld, cols, scale);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+int vllm_softmax_causal_len_bf16(void* s, long long ld, long long n_mat, int heads_per_batch, int T, const int* lens,
+                                 float scale, void* stream) {
+  if (n_mat < 0 || T <= 0 || T % 8 || ld < T || ld % 8 || heads_per_batch <= 0 || n_mat % heads_per_batch) return VLLM_EINVAL;
+  if (n_mat == 0) return VLLM_OK;
+  if (!s || !lens) return VLLM_EINVAL;
+  if (!vllm_aligned(s, 16)) return VLLM_EALIGN;
+  const long long rows = n_mat * T;
+  if (rows > 2147483647LL) return VLLM_EUNSUPPORTED;
+  return with_vpt<256, 1, 2, 4>(T / 8, [&](auto vpt, auto) {
+    softmax_causal_kernel<decltype(vpt)::value><<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)s, ld, T, scale,
+                                                                                                lens, heads_per_batch);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  });
+}
+
+int vllm_head_stack_qkv_pad_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int tokens_pad,
+                                 int nq, int nkv, int head_dim, int to_stacked, void* stream) {
+  if (batch < 0 || tokens < 0 || tokens_pad < tokens || nq <= 0 || nkv < 0 || head_dim <= 0 || (nkv && nq % nkv))
+    return VLLM_EINVAL;
+  if (ld < (long long)(nq + 2 * nkv) * head_dim) return VLLM_EINVAL;
+  const long long n_vec = (long long)batch * tokens_pad * (nq + 2 * nkv) * (head_dim / 8);
+  if (n_vec == 0) return VLLM_OK;
+  if (!packed || !q || (nkv && (!k || !v))) return VLLM_EINVAL;
+  if (head_dim % 8) return VLLM_EUNSUPPORTED;
+  if (ld % 8 || !vllm_aligned(packed, 16) || !vllm_aligned(q, 16) || !vllm_aligned(k, 16) || !vllm_aligned(v, 16))
+    return VLLM_EALIGN;
+  long long blocks = (n_vec + 255) / 256;
+  const long long cap = (long long)vllm_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  head_stack_qkv_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((uint4*)packed, ld / 8, (uint4*)q, (uint4*)k,
+                                                                           (uint4*)v, batch, tokens, tokens_pad, nq, nkv,
+                                                                           head_dim / 8, to_stacked ? 1 : 0, n_vec);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+static int gelu_launch(bool backward, const void* u, long long ldu, const void* dy, long long lddy, void* out, long long ldo,
+                       long long rows, int cols, void* stream) {
+  if (rows < 0 || cols <= 0 || cols % 8) return VLLM_EINVAL;
+  if (rows == 0) return VLLM_OK;
+  if (!u || !out || (backward && !dy)) return VLLM_EINVAL;
+  if (ldu % 8 || ldo % 8 || (backward && lddy % 8) || !vllm_aligned(u, 16) || !vllm_aligned(out, 16) ||
+      (backward && !vllm_aligned(dy, 16)))
+    return VLLM_EALIGN;
+  long long blocks = (rows * (cols / 8) + 255) / 256;
+  const long long cap = (long long)vllm_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  if (backward)
+    gelu_kernel<true><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)u, ldu, (const __nv_bfloat16*)dy,
+                                                                          lddy, (__nv_bfloat16*)out, ldo, rows, cols);
+  else
+    gelu_kernel<false><<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)u, ldu, nullptr, 0,
+                                                                           (__nv_bfloat16*)out, ldo, rows, cols);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+int vllm_gelu_fwd_bf16(const void* u, long long ldu, void* y, long long ldy, long long rows, int cols, void* stream) {
+  return gelu_launch(false, u, ldu, nullptr, 0, y, ldy, rows, cols, stream);
+}
+
+int vllm_gelu_bwd_bf16(const void* u, long long ldu, const void* dy, long long lddy, void* dx, long long lddx, long long rows,
+                       int cols, void* stream) {
+  return gelu_launch(true, u, ldu, dy, lddy, dx, lddx, rows, cols, stream);
+}
+
+int vllm_bias_grad_bf16(const void* dy, long long ldy, float* dbias, float* partials, int n_partials, long long rows, int cols,
+                        void* stream) {
+  if (rows < 0 || cols <= 0 || cols % 8) return VLLM_EINVAL;
+  if (!dbias) return VLLM_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    return (int)cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)cols, st);
+  }
+  if (!dy || !partials) return VLLM_EINVAL;
+  if (ldy % 8 || !vllm_aligned(dy, 16) || !vllm_aligned(partials, 16)) return VLLM_EALIGN;
+  const int rows_per_cta = (int)((rows + (long long)vllm_num_sms() * 8 - 1) / ((long long)vllm_num_sms() * 8));
+  const int blocks = rmsnorm_bwd_ctas(rows);
+  if (n_partials < blocks) return VLLM_EINVAL;
+  colsum_rows_kernel<<<dim3((unsigned)blocks, (unsigned)((cols / 8 + 255) / 256)), 256, 0, st>>>(
+      (const __nv_bfloat16*)dy, ldy, rows, cols, rows_per_cta, partials);
+  VLLM_CHECK_LAUNCH();
+  colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials, dbias, blocks, cols);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
+}
+
+int vllm_layernorm_bwd_wb_bf16(const void* x, long long ldx, const void* dy, long long ldy, float* dweight, float* dbias,
+                               float* partials, int n_partials, long long rows, int cols, float eps, void* stream) {
+  if (rows < 0 || cols <= 0 || cols % 8) return VLLM_EINVAL;
+  if (!dweight || !dbias) return VLLM_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    const cudaError_t e = cudaMemsetAsync(dweight, 0, sizeof(float) * (size_t)cols, st);
+    return (int)(e != cudaSuccess ? e : cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)cols, st));
+  }
+  if (!x || !dy || !partials) return VLLM_EINVAL;
+  if (ldx % 8 || ldy % 8 || !vllm_aligned(x, 16) || !vllm_aligned(dy, 16) || !vllm_aligned(partials, 16)) return VLLM_EALIGN;
+  const int rows_per_cta = (int)((rows + (long long)vllm_num_sms() * 8 - 1) / ((long long)vllm_num_sms() * 8));
+  const int blocks = rmsnorm_bwd_ctas(rows);
+  if (n_partials < blocks) return VLLM_EINVAL;
+  return with_vpt<256, 1, 2, 4, 8>(cols / 8, [&](auto vpt, auto) {
+    layernorm_bwd_wb_kernel<decltype(vpt)::value><<<(unsigned)blocks, 256, 0, st>>>(
+        (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)dy, ldy, rows, cols, eps, rows_per_cta, partials);
+    VLLM_CHECK_LAUNCH();
+    colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials, dweight, blocks, cols);
+    VLLM_CHECK_LAUNCH();
+    colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials + (size_t)blocks * cols, dbias, blocks, cols);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  });
+}
+
+int vllm_assemble_embeds_bwd_bf16(const int* dest, const int* order, long long n, const void* d_embeds, int hidden,
+                                  void* d_sources, long long source_rows, void* stream) {
+  if (n < 0 || source_rows < 0 || hidden <= 0 || hidden % 8) return VLLM_EINVAL;
+  if (source_rows == 0) return VLLM_OK;
+  if (!d_sources || (n > 0 && (!dest || !order || !d_embeds))) return VLLM_EINVAL;
+  if (!vllm_aligned(d_sources, 16) || (n > 0 && !vllm_aligned(d_embeds, 16))) return VLLM_EALIGN;
+  long long blocks = source_rows;
+  const long long cap = (long long)vllm_num_sms() * 32;
+  if (blocks > cap) blocks = cap;
+  segment_sum_rows_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(dest, order, n, (const __nv_bfloat16*)d_embeds,
+                                                                              hidden, (__nv_bfloat16*)d_sources, source_rows);
   VLLM_CHECK_LAUNCH();
   return VLLM_OK;
 }

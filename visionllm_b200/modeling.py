@@ -321,7 +321,9 @@ class B200VisionLLMv2Model(nn.Module):
             raise RuntimeError("rows carry different numbers of tool tokens: the reference cannot stack them either (mv2.py:526)")
         return torch.stack(new_ids, 0), torch.stack(new_emb, 0)
 
-    def encode_images(self, images):
+    def vision_hidden_state(self, images):
+        """mv2.py:559-572: the ViT over every image / tile -> (hidden_states[vis_output_layer] [tiles, 1 + tokens, C], tiles
+        per sample or None, the ViT outputs)."""
         if isinstance(images, (list, tuple)):                      # 'anyres': bs x [1 + n_split, 3, h, w]
             images = [x.unsqueeze(0) if x.ndim == 3 else x for x in images]
             split_sizes = [im.shape[0] for im in images]
@@ -329,7 +331,10 @@ class B200VisionLLMv2Model(nn.Module):
         else:
             split_sizes, concat = None, images
         outs = self.vis_encoder(concat, output_hidden_states=True)
-        hs = outs.hidden_states[getattr(self.config, "vis_output_layer", -2)]
+        return outs.hidden_states[getattr(self.config, "vis_output_layer", -2)], split_sizes, outs
+
+    def encode_images(self, images):
+        hs, split_sizes, outs = self.vision_hidden_state(images)
         if (self.use_pixelshuffle and FUSED_SEQUENCE and hs.is_cuda and hs.dtype == torch.bfloat16
                 and self.llm.dtype == torch.bfloat16 and hs.stride(2) == 1):
             # CLS slice + pixel shuffle (+ the LayerNorm that opens internvl_mlp) in ONE pass: the projector's A operand
@@ -380,6 +385,24 @@ class B200VisionLLMv2Model(nn.Module):
         tq.view(B, mx * self.num_embs, C)[b, rank] = hidden_states[b, p]
         tm[b, rank // self.num_embs] = True
         return tq, tm
+
+    # ---- freezing (mv2.py:286-300; the reference's train.py calls these by name) ----------------------------------
+    def freeze_vis_encoder(self):
+        self.vis_encoder.requires_grad_(False)
+
+    def freeze_llm(self):
+        self.llm.requires_grad_(False)
+
+    def freeze_vl_bridge(self):
+        self.vl_bridge.requires_grad_(False)
+
+    def freeze_region_encoder(self):
+        if getattr(self, "region_encoder", None) is not None:
+            self.region_encoder.requires_grad_(False)
+
+    def freeze_emb_embeddings(self):
+        self.emb_embeddings_det.requires_grad_(False)
+        self.emb_embeddings_pose.requires_grad_(False)
 
     # ---- forward -------------------------------------------------------------------------------
     @torch.no_grad()

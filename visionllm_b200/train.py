@@ -31,7 +31,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib, ops
-from .llama import rope_tables
+from .llama import right_padding_lengths, rope_tables
 
 
 # ---- thin wrappers over the C-ABI row kernels ------------------------------------------------------------------------
@@ -67,6 +67,80 @@ def swiglu_bwd(gu, dh):
                                              dgu.stride(0), rows, two_i // 2, ops._stream())
     _lib.check(rc, "vllm_swiglu_bwd_bf16")
     return dgu
+
+
+def _partials(rows, cols, n, device):
+    n_part = _lib.lib().vllm_rmsnorm_bwd_partials(rows)
+    return n_part, torch.empty((n * max(n_part, 1), cols), dtype=torch.float32, device=device)
+
+
+def gelu_fwd(u):
+    y = torch.empty_like(u)
+    with torch.cuda.device(u.device):
+        rc = _lib.lib().vllm_gelu_fwd_bf16(u.data_ptr(), u.stride(0), y.data_ptr(), y.stride(0), u.shape[0], u.shape[1], ops._stream())
+    _lib.check(rc, "vllm_gelu_fwd_bf16")
+    return y
+
+
+def gelu_bwd(u, dy):
+    dx = torch.empty_like(u)
+    with torch.cuda.device(u.device):
+        rc = _lib.lib().vllm_gelu_bwd_bf16(u.data_ptr(), u.stride(0), dy.data_ptr(), dy.stride(0), dx.data_ptr(), dx.stride(0),
+                                           u.shape[0], u.shape[1], ops._stream())
+    _lib.check(rc, "vllm_gelu_bwd_bf16")
+    return dx
+
+
+def bias_grad(dy2):
+    """fp32 column sums of dy [rows, N] (bf16, unit inner stride), in a fixed order (vllm_bias_grad_bf16)."""
+    rows, cols = dy2.shape
+    n_part, part = _partials(rows, cols, 1, dy2.device)
+    db = torch.empty(cols, dtype=torch.float32, device=dy2.device)
+    with torch.cuda.device(dy2.device):
+        rc = _lib.lib().vllm_bias_grad_bf16(dy2.data_ptr(), dy2.stride(0), db.data_ptr(), part.data_ptr(), n_part, rows, cols,
+                                            ops._stream())
+    _lib.check(rc, "vllm_bias_grad_bf16")
+    return db
+
+
+def layernorm_bwd_wb(x2, dy2, eps):
+    """nn.LayerNorm weight / bias gradients (fp32, fixed summation order; vllm_layernorm_bwd_wb_bf16) -- no dx."""
+    rows, cols = x2.shape
+    n_part, part = _partials(rows, cols, 2, x2.device)
+    dw = torch.empty(cols, dtype=torch.float32, device=x2.device)
+    db = torch.empty(cols, dtype=torch.float32, device=x2.device)
+    with torch.cuda.device(x2.device):
+        rc = _lib.lib().vllm_layernorm_bwd_wb_bf16(x2.data_ptr(), x2.stride(0), dy2.data_ptr(), dy2.stride(0), dw.data_ptr(),
+                                                   db.data_ptr(), part.data_ptr(), n_part, rows, cols, float(eps), ops._stream())
+    _lib.check(rc, "vllm_layernorm_bwd_wb_bf16")
+    return dw, db
+
+
+def assemble_embeds_bwd(plan, d_embeds, source_rows, wanted):
+    """Gradients of ops.assemble_embeds' sources from d(inputs_embeds) [B, L, C]: `source_rows` = rows of (token table, det
+    table, pose table, image features), `wanted` = which of them need a gradient.  Positions are sorted stably by destination
+    row (torch.sort, glue) and one segment-sum kernel (vllm_assemble_embeds_bwd_bf16) writes every wanted source: fp32 sums
+    in position order, rows no position names exact 0.  Returns one tensor (or None) per source."""
+    C = d_embeds.shape[-1]
+    base, offs = 0, []
+    for n, w in zip(source_rows, wanted):
+        offs.append(base if w else None)
+        base += n if w else 0
+    if base == 0:
+        return [None] * 4
+    big = torch.iinfo(torch.int32).max                             # positions of unwanted sources sort past every row
+    lut = torch.tensor([o if o is not None else big for o in offs], dtype=torch.int64, device=d_embeds.device)
+    dest = torch.minimum(lut[plan.kind.reshape(-1).long()] + plan.row.reshape(-1).long(), lut.new_tensor(big))
+    dest, order = torch.sort(dest.to(torch.int32), stable=True)
+    order = order.to(torch.int32)
+    dy = d_embeds.reshape(-1, C)
+    dy = dy if dy.is_contiguous() and dy.dtype == torch.bfloat16 else dy.to(torch.bfloat16).contiguous()
+    out = torch.empty((base, C), dtype=torch.bfloat16, device=d_embeds.device)
+    with torch.cuda.device(out.device):
+        rc = _lib.lib().vllm_assemble_embeds_bwd_bf16(dest.data_ptr(), order.data_ptr(), dest.numel(), dy.data_ptr(), C,
+                                                      out.data_ptr(), base, ops._stream())
+    _lib.check(rc, "vllm_assemble_embeds_bwd_bf16")
+    return [out[o:o + n] if o is not None else None for o, n in zip(offs, source_rows)]
 
 
 def head_stack(t, B, T, parts, H, D, to_stacked):
@@ -112,40 +186,78 @@ def gemm_batched(a, b, n_batch, M, N, K, a_mn=False, b_mn=False, causal=0, out_d
     return out
 
 
-def attention_backward_packed(qkv5, do, scale):
+def head_stack_qkv_pad(rows, nq, nkv, D, T_pad, stacks=None):
+    """head_stack_qkv with T_pad >= T rows per (batch, head) matrix (vllm_head_stack_qkv_pad_bf16): rows T .. T_pad - 1 of
+    every stacked matrix are zeros; the inverse skips them.  nkv = 0 stacks the nq heads of a plain [B, T, nq D] tensor."""
+    B, T = rows.shape[0], rows.shape[1]
+    to_stacked = stacks is None
+    if to_stacked:
+        stacks = torch.empty(((nq + 2 * nkv) * B * T_pad, D), dtype=rows.dtype, device=rows.device)
+    nq_rows, nkv_rows = B * nq * T_pad, B * nkv * T_pad
+    q, k, v = stacks[:nq_rows], stacks[nq_rows:nq_rows + nkv_rows], stacks[nq_rows + nkv_rows:]
+    with torch.cuda.device(rows.device):
+        rc = _lib.lib().vllm_head_stack_qkv_pad_bf16(rows.data_ptr(), rows.stride(1), q.data_ptr(),
+                                                     k.data_ptr() if nkv else None, v.data_ptr() if nkv else None, B, T, T_pad,
+                                                     nq, nkv, D, 1 if to_stacked else 0, ops._stream())
+    _lib.check(rc, "vllm_head_stack_qkv_pad_bf16")
+    return stacks if to_stacked else rows
+
+
+def attention_backward_packed(qkv5, do, scale, seqlens=None):
     """Backward of causal softmax(q k^T * scale) v for the PACKED projection output qkv5 [B, T, G + 2, nkv, D] (bf16: the
     nq = G * nkv query heads, then the nkv key heads, then the nkv value heads of a row; q head i attends with KV head
     i // G, as HF's repeat_kv; MHA is G = 1, [B, T, 3, H, D]) and do [B, T, nq*D].  Returns d(qkv5) in the same packed
     layout.  The (batch, head) matrices are stacked along rows for the block-diagonal batched GEMMs by ONE copy of qkv5
     (and one of do); the three gradient GEMMs write one stacked buffer that ONE copy turns back into the packed layout.
     Grouped-query attention needs no repeated K / V: S, dP and dQ read KV matrix i // G, and dK, dV reduce over the G
-    query matrices of a KV head inside one GEMM (fp32 accumulation, one rounding)."""
+    query matrices of a KV head inside one GEMM (fp32 accumulation, one rounding).
+
+    seqlens (int32 [B], right padding) or a T that is not a multiple of 256 takes the padded form: every matrix is stacked
+    with T_pad = roundup(T, 256) rows (zeros past T), the softmax gives P = 0 for keys j >= seqlens[b] (HF's mask: key j is
+    visible to query i iff j <= i and j < len, for every query row), and with P = 0 the softmax backward gives dS = 0 there,
+    so the same five GEMMs and dS kernel serve."""
     B, T, parts, nkv, D = qkv5.shape
     G = parts - 2
-    if G < 1 or T % 256 or D % 64:
-        raise RuntimeError("attention_backward: sequence length must be a multiple of 256 and head_dim of 64")
+    if G < 1 or D % 64:
+        raise RuntimeError("attention_backward: head_dim must be a multiple of 64")
+    padded = seqlens is not None or T % 256 != 0
+    Tp = (T + 255) // 256 * 256
     nq = G * nkv
     BQ, BKV = B * nq, B * nkv
     rows = qkv5.reshape(B, T, -1)                                               # a view for the decoder's packed projection
     if rows.stride(2) != 1 or rows.stride(1) % 8 or rows.data_ptr() % 16:
         rows = rows.contiguous()
-    stk = head_stack_qkv(rows, nq, nkv, D)                                      # Q | K | V stacks, [(b, h), T, D] each
-    qs, ks, vs = stk[:BQ * T], stk[BQ * T:(BQ + BKV) * T], stk[(BQ + BKV) * T:]
-    dos = head_stack(do, B, T, 1, nq, D, True).view(BQ * T, D)
+    if padded:
+        stk = head_stack_qkv_pad(rows, nq, nkv, D, Tp)
+        dos = head_stack_qkv_pad(do.reshape(B, T, nq * D).contiguous(), nq, 0, D, Tp)
+    else:
+        stk = head_stack_qkv(rows, nq, nkv, D)                                  # Q | K | V stacks, [(b, h), T, D] each
+        dos = head_stack(do, B, T, 1, nq, D, True).view(BQ * T, D)
+    qs, ks, vs = stk[:BQ * Tp], stk[BQ * Tp:(BQ + BKV) * Tp], stk[(BQ + BKV) * Tp:]
     L_ = _lib.lib()
-    p = gemm_batched(qs, ks, BQ, T, T, D, causal=1, group=G)                     # S = Q K^T, tiles above the diagonal skipped
+    p = gemm_batched(qs, ks, BQ, Tp, Tp, D, causal=1, group=G)                   # S = Q K^T, tiles above the diagonal skipped
     with torch.cuda.device(qkv5.device):
-        _lib.check(L_.vllm_softmax_causal_bf16(p.data_ptr(), p.stride(0), BQ, T, float(scale), ops._stream()), "vllm_softmax_causal_bf16")
-    dp = gemm_batched(dos, vs, BQ, T, T, D, causal=1, group=G)                   # dP = dO V^T
+        if padded:
+            # lengths past T are T, as in the forward kernel (min(seqlens[b], Tk)): the zero rows T .. T_pad stay masked
+            lens = (seqlens.clamp(max=T) if seqlens is not None else
+                    torch.full((B,), T, dtype=torch.int32, device=qkv5.device))
+            rc = L_.vllm_softmax_causal_len_bf16(p.data_ptr(), p.stride(0), BQ, nq, Tp, lens.data_ptr(), float(scale), ops._stream())
+            _lib.check(rc, "vllm_softmax_causal_len_bf16")
+        else:
+            _lib.check(L_.vllm_softmax_causal_bf16(p.data_ptr(), p.stride(0), BQ, T, float(scale), ops._stream()),
+                       "vllm_softmax_causal_bf16")
+    dp = gemm_batched(dos, vs, BQ, Tp, Tp, D, causal=1, group=G)                 # dP = dO V^T
     with torch.cuda.device(qkv5.device):
-        _lib.check(L_.vllm_attn_ds_bf16(p.data_ptr(), dp.data_ptr(), p.stride(0), BQ, T, float(scale), ops._stream()), "vllm_attn_ds_bf16")
+        _lib.check(L_.vllm_attn_ds_bf16(p.data_ptr(), dp.data_ptr(), p.stride(0), BQ, Tp, float(scale), ops._stream()), "vllm_attn_ds_bf16")
     ds = dp
     dstk = torch.empty_like(stk)
-    dqs, dks, dvs = dstk[:BQ * T], dstk[BQ * T:(BQ + BKV) * T], dstk[(BQ + BKV) * T:]
-    gemm_batched(p, dos, BQ, T, D, T, a_mn=True, b_mn=True, causal=2, out=dvs, group=G, reduce=True)   # dV = sum_g P_g^T dO_g
-    gemm_batched(ds, qs, BQ, T, D, T, a_mn=True, b_mn=True, causal=2, out=dks, group=G, reduce=True)   # dK = sum_g dS_g^T Q_g
-    gemm_batched(ds, ks, BQ, T, D, T, b_mn=True, causal=3, out=dqs, group=G)                            # dQ = dS K
+    dqs, dks, dvs = dstk[:BQ * Tp], dstk[BQ * Tp:(BQ + BKV) * Tp], dstk[(BQ + BKV) * Tp:]
+    gemm_batched(p, dos, BQ, Tp, D, Tp, a_mn=True, b_mn=True, causal=2, out=dvs, group=G, reduce=True)   # dV = sum_g P_g^T dO_g
+    gemm_batched(ds, qs, BQ, Tp, D, Tp, a_mn=True, b_mn=True, causal=2, out=dks, group=G, reduce=True)   # dK = sum_g dS_g^T Q_g
+    gemm_batched(ds, ks, BQ, Tp, D, Tp, b_mn=True, causal=3, out=dqs, group=G)                            # dQ = dS K
     dqkv = torch.empty((B, T, parts * nkv * D), dtype=qkv5.dtype, device=qkv5.device)
+    if padded:
+        return head_stack_qkv_pad(dqkv, nq, nkv, D, Tp, stacks=dstk).view(B, T, parts, nkv, D)
     return head_stack_qkv(dqkv, nq, nkv, D, stacks=dstk).view(B, T, parts, nkv, D)  # packed gradient
 
 
@@ -162,12 +274,12 @@ def attention_backward(q, k, v, do, scale):
 # ---- autograd Functions --------------------------------------------------------------------------------------------------
 class LinearFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, out_f32=False, residual=None):
+    def forward(ctx, x, weight, out_f32=False, residual=None, bias=None):
         ctx.save_for_backward(x, weight)
         ctx.has_res = residual is not None
         if not out_f32:
-            return ops.linear(x, weight, residual=residual)      # y = x W^T (+ residual in the GEMM epilogue)
-        assert residual is None
+            return ops.linear(x, weight, bias=bias, residual=residual)   # y = x W^T (+ bias, + residual in the GEMM epilogue)
+        assert residual is None and bias is None
         # fp32 rows need a 16-byte pitch (V = 32026 is not a multiple of 4): pad the pitch, return the [.., :V] view
         N = weight.shape[0]
         rows = x.numel() // x.shape[-1]
@@ -190,7 +302,8 @@ class LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             dw = ops.gemm_tn(dy2, x2, a_mn=True, b_mn=True, out_dtype=torch.bfloat16 if w.dtype == torch.bfloat16 else torch.float32)
             dw = dw if dw.dtype == w.dtype else dw.to(w.dtype)
-        return dx, dw, None, (dy if ctx.has_res else None)
+        db = bias_grad(dy2).to(w.dtype) if len(ctx.needs_input_grad) > 4 and ctx.needs_input_grad[4] else None
+        return dx, dw, None, (dy if ctx.has_res else None), db
 
 
 class RMSNormFn(torch.autograd.Function):
@@ -272,19 +385,22 @@ class CausalAttentionFn(torch.autograd.Function):
 class CausalAttentionPackedFn(torch.autograd.Function):
     """Causal attention on the packed projection output qkv5 [B, T, G + 2, nkv, D] (G query heads per KV head; MHA:
     [B, T, 3, H, D]): the forward reads q / k / v as strided views (no copies), the backward returns the packed gradient
-    (attention_backward_packed)."""
+    (attention_backward_packed).  seqlens: int32 [B] key lengths of a right-padded batch, or None."""
 
     @staticmethod
-    def forward(ctx, qkv5, scale):
+    def forward(ctx, qkv5, scale, seqlens=None):
         ctx.save_for_backward(qkv5)
-        ctx.scale = scale
+        ctx.scale, ctx.seqlens = scale, seqlens
         G = qkv5.shape[2] - 2
-        return ops.attention(qkv5[:, :, :G].flatten(2, 3), qkv5[:, :, G], qkv5[:, :, G + 1], causal=True, scale=scale)
+        return ops.attention(qkv5[:, :, :G].flatten(2, 3), qkv5[:, :, G], qkv5[:, :, G + 1], causal=True, scale=scale,
+                             seqlens=seqlens)
 
     @staticmethod
     def backward(ctx, dctx):
         (qkv5,) = ctx.saved_tensors
-        return attention_backward_packed(qkv5, dctx, ctx.scale), None
+        if ctx.seqlens is None:
+            return attention_backward_packed(qkv5, dctx, ctx.scale), None, None
+        return attention_backward_packed(qkv5, dctx, ctx.scale, ctx.seqlens), None, None
 
 
 class SwiGLUFn(torch.autograd.Function):
@@ -333,15 +449,15 @@ class CrossEntropyFn(torch.autograd.Function):
 
 
 # ---- the trainable decoders ---------------------------------------------------------------------------------------------
-def decoder_layer_train(x, cos, sin, neg_sin, norm1_w, norm2_w, eps, wqkv, wo, w_gate_up, w_down, nq, nkv, D):
+def decoder_layer_train(x, cos, sin, neg_sin, norm1_w, norm2_w, eps, wqkv, wo, w_gate_up, w_down, nq, nkv, D, seqlens=None):
     """fwd of one pre-norm decoder layer as autograd Functions on this repo's kernels, on the layer's (packed) weights --
     shared by the Llama and InternLM2 training wrappers, as llama.decoder_layer_forward is by the inference modules:
     RMSNorm, q|k|v GEMM + RoPE on the nq + nkv q and k heads, causal (grouped-query) attention, O GEMM (+ residual in the
-    epilogue), RMSNorm, gate|up GEMM, SwiGLU, down GEMM (+ residual)."""
+    epilogue), RMSNorm, gate|up GEMM, SwiGLU, down GEMM (+ residual).  seqlens: key lengths of a right-padded batch."""
     B, T, H = x.shape
     h = RMSNormFn.apply(x, norm1_w, eps)
     qkv = QKVRopeFn.apply(h.view(B * T, H), wqkv, cos, sin, neg_sin, nq + nkv, D).view(B, T, nq // nkv + 2, nkv, D)
-    ctx = CausalAttentionPackedFn.apply(qkv, D ** -0.5)
+    ctx = CausalAttentionPackedFn.apply(qkv, D ** -0.5, seqlens)
     x = LinearFn.apply(ctx, wo, False, x)                                             # + residual in the GEMM epilogue
     h = RMSNormFn.apply(x, norm2_w, eps)
     gu = LinearFn.apply(h, w_gate_up)
@@ -350,8 +466,9 @@ def decoder_layer_train(x, cos, sin, neg_sin, norm1_w, norm2_w, eps, wqkv, wo, w
 
 
 class _DecoderTrain(nn.Module):
-    """fwd+bwd of a decoder stack on the parameters of an inference module (shared, not copied); sequence length a multiple
-    of 256.  A subclass names the weights: layer_weights(layer) -> (norm1, norm2, wqkv, wo, w_gate_up, w_down), where
+    """fwd+bwd of a decoder stack on the parameters of an inference module (shared, not copied); any sequence length, and
+    right-padded batches through `attention_mask` (HF semantics: key j is visible to query i iff j <= i and j < len[b],
+    positions stay arange(T)).  A subclass names the weights: layer_weights(layer) -> (norm1, norm2, wqkv, wo, w_gate_up, w_down), where
     wqkv / w_gate_up are differentiable functions of the module's parameters (so the gradients land on them), and
     final_weights() -> (final norm, lm head)."""
 
@@ -362,15 +479,17 @@ class _DecoderTrain(nn.Module):
         if nq % nkv:
             raise NotImplementedError("num_attention_heads must be a multiple of num_key_value_heads")
 
-    def forward(self, inputs_embeds, labels=None):
+    def forward(self, inputs_embeds, labels=None, attention_mask=None):
         B, T, H = inputs_embeds.shape
+        seqlens = right_padding_lengths(attention_mask)                  # None when nothing is padded: the unmasked path
         pos = torch.arange(T, device=inputs_embeds.device)[None].expand(B, T)
         cos, sin = rope_tables(pos, self.D, self.theta, inputs_embeds.dtype)
         neg_sin = (-sin).contiguous()
         x = inputs_embeds
         for layer in self.layers():
             n1, n2, wqkv, wo, wgu, wdown = self.layer_weights(layer)
-            x = decoder_layer_train(x, cos, sin, neg_sin, n1, n2, self.eps, wqkv, wo, wgu, wdown, self.nq, self.nkv, self.D)
+            x = decoder_layer_train(x, cos, sin, neg_sin, n1, n2, self.eps, wqkv, wo, wgu, wdown, self.nq, self.nkv, self.D,
+                                    seqlens)
         norm_w, head_w = self.final_weights()
         hidden = RMSNormFn.apply(x, norm_w, self.eps)
         # fp32 logits like `logits.float()` (mv2.py:738), as a 2-D [B*T, V] view of a pitch-padded buffer so that the loss
@@ -451,3 +570,152 @@ class B200InternLM2ForCausalLMTrain(_DecoderTrain):
 
     def final_weights(self):
         return self.lm.model.norm.weight, self.lm.output.weight
+
+
+# ---- the multimodal chat step: vision-language bridge and sequence assembly with gradients -----------------------------
+class GeluFn(torch.autograd.Function):
+    """Exact-erf GELU (nn.GELU()) on the saved pre-activation u: y = gelu(u), du = dy * gelu'(u)."""
+
+    @staticmethod
+    def forward(ctx, u):
+        ctx.save_for_backward(u)
+        return gelu_fwd(u)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (u,) = ctx.saved_tensors
+        return gelu_bwd(u, dy.contiguous())
+
+
+class LayerNormWBFn(torch.autograd.Function):
+    """nn.LayerNorm whose input takes no gradient (the frozen ViT's features): backward gives the weight / bias gradients."""
+
+    @staticmethod
+    def forward(ctx, x2, weight, bias, eps):
+        if ctx.needs_input_grad[0]:
+            raise NotImplementedError("LayerNorm backward to its input: the vision encoder must be frozen")
+        ctx.save_for_backward(x2)
+        ctx.eps = eps
+        return ops.layernorm(x2, weight, bias, eps)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x2,) = ctx.saved_tensors
+        if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
+            return None, None, None, None
+        dw, db = layernorm_bwd_wb(x2, dy.contiguous(), ctx.eps)
+        return None, dw.to(torch.bfloat16), db.to(torch.bfloat16), None
+
+
+class AssembleEmbedsFn(torch.autograd.Function):
+    """ops.assemble_embeds with gradients for the token table, the two [EMB] tables and the image features."""
+
+    @staticmethod
+    def forward(ctx, plan, embed_w, det_w, pose_w, feats, padding_idx=None):
+        ctx.plan, ctx.padding_idx = plan, padding_idx
+        ctx.rows = (embed_w.shape[0], det_w.shape[0], pose_w.shape[0], feats.shape[0] if feats is not None else 0)
+        return ops.assemble_embeds(plan, embed_w, det_w, pose_w, feats)
+
+    @staticmethod
+    def backward(ctx, dy):
+        want = list(ctx.needs_input_grad[1:5])
+        grads = assemble_embeds_bwd(ctx.plan, dy, ctx.rows, want)
+        if grads[0] is not None and ctx.padding_idx is not None:
+            grads[0][ctx.padding_idx].zero_()                        # nn.Embedding(padding_idx=...): that row takes no gradient
+        return (None, *grads, None)
+
+
+def bridge_train(bridge, x2):
+    """The vl_bridge (modeling.build_vl_bridge: `linear`, `mlpNx_gelu`, `internvl_mlp`) as autograd Functions on x2 [rows, in]:
+    Linear = GEMM with the bias in the epilogue (dgrad / wgrad GEMMs, bias gradient kernel); a GELU after a Linear stores the
+    pre-activation and applies GELU in its own pass; the LayerNorm of internvl_mlp runs unfused (weight / bias gradients)."""
+    from .modeling import BridgeLayerNorm, BridgeLinear
+    mods = [bridge] if isinstance(bridge, BridgeLinear) else list(bridge)
+    x = x2
+    for m in mods:
+        if isinstance(m, BridgeLinear):
+            x = LinearFn.apply(x, m.weight, False, None, m.bias)
+        elif isinstance(m, nn.GELU):
+            if m.approximate != "none":
+                raise NotImplementedError("vl_bridge GELU: only the exact-erf form")
+            x = GeluFn.apply(x)
+        elif isinstance(m, BridgeLayerNorm):
+            x = LayerNormWBFn.apply(x, m.weight, m.bias, m.eps)
+        else:
+            raise NotImplementedError(f"vl_bridge module {type(m).__name__} has no training path")
+    return x
+
+
+def _require_cuda_bf16(*tensors):
+    """The step runs on CUDA tensors, floating-point ones in bfloat16."""
+    for t in tensors:
+        if t is not None and (not t.is_cuda or (t.is_floating_point() and t.dtype != torch.bfloat16)):
+            raise NotImplementedError("the training step runs on CUDA tensors, floating-point ones in bfloat16")
+
+
+def _bridge_input(model, hs):
+    """[tiles, 1 + tokens, C] ViT hidden state -> the bridge's input rows (CLS dropped, pixel shuffle when configured)."""
+    if model.use_pixelshuffle:
+        x = ops.pixel_shuffle_rows(hs, 1)
+    else:
+        x = hs[:, 1:].contiguous()
+    return x.reshape(-1, x.shape[-1])
+
+
+class B200VisionLLMv2ModelTrain(nn.Module):
+    """fwd+bwd of the reference's chat training step (train.py: `model(**batch)` then `loss.backward()`) on the parameters of
+    a `B200VisionLLMv2Model` (shared, not copied): the frozen vision encoder under no_grad, the vl_bridge, the sequence
+    assembly (token table, [EMB] tables, image features) and the LLM decoder with gradients, on right-padded batches.
+    Modules frozen with the composite's freeze_* methods get no gradient and cost no weight-gradient GEMM.
+    Refused (NotImplementedError): a trainable vision encoder, atom-tool losses (`targets`, `images_aug`), region-encoder
+    training (`regions`), the [EMB] insert form, KV caches, caller-provided `inputs_embeds`, non-CUDA / non-bf16 batches."""
+
+    def __init__(self, model):
+        super().__init__()
+        from .internlm2 import B200InternLM2ForCausalLM
+        self.model = model
+        lm = model.llm
+        self.llm_train = B200InternLM2ForCausalLMTrain(lm) if isinstance(lm, B200InternLM2ForCausalLM) else B200LlamaForCausalLMTrain(lm)
+
+    def forward(self, input_ids=None, inputs_embeds=None, attention_mask=None, images=None, images_aug=None, img_metas=None,
+                targets=None, labels=None, past_key_values=None, use_cache=False, output_attentions=False,
+                output_hidden_states=False, return_dict=True, regions=None, num_splits=None, **unused):
+        from .modeling import IGNORE_INDEX, VisionLLMv2ModelOutput
+        m = self.model
+        if past_key_values is not None or use_cache:
+            raise NotImplementedError("training with a KV cache")
+        if targets is not None or images_aug is not None:
+            raise NotImplementedError("atom-tool losses (detection / pose / generation targets) have no training path")
+        if regions is not None:
+            raise NotImplementedError("region-encoder training has no training path")
+        if inputs_embeds is not None or input_ids is None:
+            raise NotImplementedError("the training step takes input_ids (the reference's collator batch)")
+        _require_cuda_bf16(input_ids, m.llm.get_input_embeddings().weight,
+                           *(images if isinstance(images, (list, tuple)) else [images]))
+        feats, split_sizes = None, False
+        if images is not None:
+            if any(p.requires_grad for p in m.vis_encoder.parameters()):
+                raise NotImplementedError("a trainable vision encoder: call freeze_vis_encoder() (the reference's default)")
+            with torch.no_grad():
+                hs, split_sizes, _ = m.vision_hidden_state(images)
+            feats = bridge_train(m.vl_bridge, _bridge_input(m, hs))
+        tokens_per_tile = 0
+        if feats is not None:
+            tiles = sum(split_sizes) if split_sizes is not None else hs.shape[0]
+            tokens_per_tile = feats.shape[0] // tiles
+        plan = ops.seq_index(input_ids, (m.det_tool_id, m.seg_tool_id, m.grd_tool_id), (m.pose_tool_id,), m.emb_token_id,
+                             m.num_embs, m.imp_token_id, split_sizes if images is not None else False, tokens_per_tile)
+        status = int(plan.status.item())
+        if status & 1:
+            raise NotImplementedError("the [EMB] insert form (tool tokens without pre-placed [EMB] slots) has no training path")
+        if status & 2:
+            raise RuntimeError("image token count mismatch between the <im_patch> slots and the ViT tokens")
+        table = m.llm.get_input_embeddings()
+        # the reference's token table is nn.Embedding(..., padding_idx=pad_token_id) (HF Llama, InternLM2)
+        pad = table.padding_idx if table.padding_idx is not None else getattr(m.llm.config, "pad_token_id", None)
+        embeds = AssembleEmbedsFn.apply(plan, table.weight, m.emb_embeddings_det.weight, m.emb_embeddings_pose.weight, feats,
+                                        pad if pad is not None and 0 <= pad < table.weight.shape[0] else None)
+        if labels is not None:                                                               # mv2.py:740-757
+            labels[(labels >= m.emb_token_id) & (labels <= m.emb_token_id + m.num_embs - 1)] = IGNORE_INDEX
+        loss, logits, hidden = self.llm_train(embeds, labels=labels, attention_mask=attention_mask)
+        return VisionLLMv2ModelOutput(loss=loss, logits=logits, last_hidden_state=hidden, input_ids=plan.new_ids)
