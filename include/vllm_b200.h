@@ -503,6 +503,27 @@ int vllm_layernorm_bwd_wb_bf16(const void* x, long long ldx, const void* dy, lon
  * table gradients and the gather of d(image features) (each feature row is named at most once: an exact copy). */
 int vllm_assemble_embeds_bwd_bf16(const int* dest, const int* order, long long n, const void* d_embeds, int hidden,
                                   void* d_sources, long long source_rows, void* stream);
+/* Backward of the region encoder (csrc/train_ops.cu).
+ *   vllm_layernorm_gelu_bwd_bf16  backward of vllm_layernorm_gelu_bf16 (y = gelu(z), z = (x - mean) * rstd * w + b): the
+ *        statistics and z are recomputed with the forward's bits; g = dy * gelu'(z), n = (x - mean) * rstd;
+ *        dx = rstd * (w g - mean(w g) - n * mean(w g n)) (bf16, one rounding), dweight = sum g n, dbias = sum g (fp32,
+ *        fixed order through partials [2 n_partials, cols], n_partials >= vllm_layernorm_gelu_bwd_partials(rows)).  The
+ *        forward's shapes: cols % 8 == 0 and cols <= 16384 (else VLLM_EUNSUPPORTED); rows = 0 zeroes dweight and dbias.
+ *   vllm_point_pool_bwd_bf16  backward of the grid_sample point pooling (one-level MSDA sampling of n_points points per
+ *        region with weights 1 / 0, a sum and a division by the count) for `levels` feature levels sharing one map:
+ *        loc [levels, regions, n_points, 2] fp32 (x, y in [0, 1]), weight [levels, regions, n_points] fp32, counts
+ *        [levels, regions] fp32 (the forward's sums of the weights), grad [levels, regions, channels] bf16 ->
+ *        d_map [regions, height * width, channels] bf16 = sum_l a_l (x) grad_l / count_l, where a_l is the splat density
+ *        of the level's points (their bilinear corner weights times their weight, msda_geom's sampling rule, summed over
+ *        the points in index order).  density: fp32 workspace [levels, regions, height * width].  No float atomics:
+ *        run-to-run identical.  A level with count 0 adds exact 0. */
+long long vllm_layernorm_gelu_bwd_partials(long long rows);
+int vllm_layernorm_gelu_bwd_bf16(const void* x, long long ldx, const void* weight, const void* bias, const void* dy,
+                                 long long ldy, void* dx, long long lddx, float* dweight, float* dbias, float* partials,
+                                 long long n_partials, long long rows, int cols, float eps, void* stream);
+int vllm_point_pool_bwd_bf16(const float* loc, const float* weight, const float* counts, int n_points, const void* grad,
+                             int levels, int regions, int height, int width, int channels, float* density, void* d_map,
+                             void* stream);
 
 /* ---- sequence assembly of VisionLLMv2Model.forward (SURVEY 8f rank 2, 8a-a7/a9; csrc/seqglue.cu) -----------------
  * vllm_seq_index: ONE pass over input_ids [batch, seq_len] (int64, device) producing

@@ -69,6 +69,9 @@ _SIGNATURES = {
     "vllm_bias_grad_bf16": (ci, [vp, cll, vp, vp, ci, cll, ci, vp]),
     "vllm_layernorm_bwd_wb_bf16": (ci, [vp, cll, vp, cll, vp, vp, vp, ci, cll, ci, cf, vp]),
     "vllm_assemble_embeds_bwd_bf16": (ci, [vp, vp, cll, vp, ci, vp, cll, vp]),
+    "vllm_layernorm_gelu_bwd_partials": (cll, [cll]),
+    "vllm_layernorm_gelu_bwd_bf16": (ci, [vp, cll, vp, vp, vp, cll, vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),
+    "vllm_point_pool_bwd_bf16": (ci, [vp, vp, vp, ci, vp, ci, ci, ci, ci, ci, vp, vp, vp]),
     "vllm_gemm_set_variant": (ci, [ci]),
     "vllm_rmsnorm_bf16": (ci, [vp, cll, vp, vp, cll, cll, ci, cf, vp]),
     "vllm_layernorm_bf16": (ci, [vp, cll, vp, vp, vp, cll, cll, ci, cf, vp]),

@@ -12,6 +12,7 @@
 //   ce_loss_kernel         visionllmv2/model/modeling_visionllmv2.py:741-757: CrossEntropyLoss (mean over labels != -100) of
 //                          fp32 logits rows vs int64 labels; writes the loss sum and dlogits = (softmax - onehot) / n_valid.
 #include "rows.cuh"
+#include "msda_common.cuh"
 
 namespace {
 
@@ -452,6 +453,161 @@ layernorm_bwd_wb_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, cons
   }
 }
 
+// Backward of vllm_layernorm_gelu_bf16 (y = gelu(z), z = n w + b, n = (x - mean) rstd; the region encoder's LayerNorm2d ->
+// GELU): the statistics are recomputed by ln_stats at the forward's (VPT, TPR), z by ln_apply, so both are the forward's
+// bits.  g = dy gelu'(z);  dx = rstd (w g - mean(w g) - n mean(w g n)), one rounding;  dweight += g n, dbias += g.
+// A row is owned by TPR threads, a CTA holds 256 / TPR row slots; slot s owns rows [s rps, (s + 1) rps) in order and
+// writes its sums to rows s (dweight) and n_slots + s (dbias) of partials [2 n_slots, cols] (colsum_partials_kernel).
+// Every slot of a CTA runs rps iterations (the row reductions of TPR > 32 synchronise the CTA); a row past the end is
+// zeros and neither stored nor summed.
+template <int VPT, int TPR>
+__global__ void __launch_bounds__(256)
+layernorm_gelu_bwd_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __nv_bfloat16* __restrict__ w,
+                          const __nv_bfloat16* __restrict__ b, const __nv_bfloat16* __restrict__ dy, long long ldy,
+                          __nv_bfloat16* __restrict__ dx, long long lddx, long long rows, int cols, float eps, int rps,
+                          long long n_slots, float* __restrict__ partials) {
+  __shared__ float sh[8];
+  const int tr = threadIdx.x % TPR, nvec = cols / 8;
+  const long long slot = (long long)blockIdx.x * (256 / TPR) + threadIdx.x / TPR;
+  const bool slot_ok = slot < n_slots;
+  float gacc[VPT][8], bacc[VPT][8];
+#pragma unroll
+  for (int i = 0; i < VPT; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) gacc[i][j] = bacc[i][j] = 0.f;
+  for (int k = 0; k < rps; ++k) {
+    const long long row = slot * rps + k;
+    const bool ok = slot_ok && row < rows;
+    uint4 xr[VPT];
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int v = tr + i * TPR;
+      xr[i] = (ok && v < nvec) ? *(reinterpret_cast<const uint4*>(x + row * ldx) + v) : make_uint4(0u, 0u, 0u, 0u);
+    }
+    const float2 st = ln_stats<VPT, TPR, 256>(xr, cols, eps, sh);
+    float s1 = 0.f, s2 = 0.f;                                 // sum w g, sum w g n
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int v = tr + i * TPR;
+      if (ok && v < nvec) {
+        float f[8], z[8], g[8], wv[8];
+        unpack8(xr[i], f); unpack8(__ldg(reinterpret_cast<const uint4*>(w) + v), wv);
+        unpack8(*(reinterpret_cast<const uint4*>(dy + row * ldy) + v), g);
+        ln_apply(xr[i], w, b, v, st, z);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float n = (f[j] - st.x) * st.y;
+          g[j] *= gelu_erf_grad(z[j]);
+          gacc[i][j] += g[j] * n;
+          bacc[i][j] += g[j];
+          s1 += wv[j] * g[j];
+          s2 += wv[j] * g[j] * n;
+        }
+      }
+    }
+    const float m1 = row_sum<TPR, true, 256>(s1, sh) / cols;
+    const float m2 = row_sum<TPR, true, 256>(s2, sh) / cols;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int v = tr + i * TPR;
+      if (ok && v < nvec) {
+        float f[8], z[8], g[8], wv[8], o[8];
+        unpack8(xr[i], f); unpack8(__ldg(reinterpret_cast<const uint4*>(w) + v), wv);
+        unpack8(*(reinterpret_cast<const uint4*>(dy + row * ldy) + v), g);
+        ln_apply(xr[i], w, b, v, st, z);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float n = (f[j] - st.x) * st.y;
+          o[j] = st.y * (wv[j] * (g[j] * gelu_erf_grad(z[j])) - m1 - n * m2);
+        }
+        *(reinterpret_cast<uint4*>(dx + row * lddx) + v) = pack8(o);
+      }
+    }
+  }
+  if (!slot_ok) return;
+#pragma unroll
+  for (int i = 0; i < VPT; ++i) {
+    const int v = tr + i * TPR;
+    if (v < nvec) {
+      float* pg = partials + (size_t)slot * cols + v * 8;
+      float* pb = partials + (size_t)(n_slots + slot) * cols + v * 8;
+      *reinterpret_cast<float4*>(pg) = make_float4(gacc[i][0], gacc[i][1], gacc[i][2], gacc[i][3]);
+      *reinterpret_cast<float4*>(pg + 4) = make_float4(gacc[i][4], gacc[i][5], gacc[i][6], gacc[i][7]);
+      *reinterpret_cast<float4*>(pb) = make_float4(bacc[i][0], bacc[i][1], bacc[i][2], bacc[i][3]);
+      *reinterpret_cast<float4*>(pb + 4) = make_float4(bacc[i][4], bacc[i][5], bacc[i][6], bacc[i][7]);
+    }
+  }
+}
+
+// Backward of the region encoder's point pooling (the MSDA kernel with one level, point weights pw, then a sum over the
+// points and a division by their count).  Splat density of (level l, region r): a[l, r, pixel] = sum over the points in
+// index order of pw * (bilinear corner weight of the point at that pixel), fp32, the corner geometry of msda_geom (the
+// forward's sampling rule; corners outside the map take nothing).  One thread per pixel, the points staged 256 at a time
+// in shared memory: a gather, so the sum has one order and no atomics.
+__global__ void __launch_bounds__(256)
+point_density_kernel(const float* __restrict__ loc, const float* __restrict__ pw, int n_pts, int R, int H, int W,
+                     float* __restrict__ density) {
+  __shared__ int s_hl[256], s_wl[256];
+  __shared__ float s_lh[256], s_lw[256], s_pw[256];
+  const int r = blockIdx.y, l = blockIdx.z;
+  const int p = blockIdx.x * 256 + threadIdx.x;
+  const int py = p / W, px = p - (p / W) * W;
+  const long long base = ((long long)l * R + r) * n_pts;
+  float a = 0.f;
+  for (int c0 = 0; c0 < n_pts; c0 += 256) {
+    const int i = c0 + threadIdx.x;
+    __syncthreads();
+    if (i < n_pts) {
+      const float2 xy = *reinterpret_cast<const float2*>(loc + 2 * (base + i));
+      const MsdaGeom<float> g = msda_geom<float>(xy.x, xy.y, H, W);
+      const bool in = g.mask & 1;
+      s_hl[threadIdx.x] = in ? g.h_low : INT_MIN / 2;          // a sample outside the map touches no pixel
+      s_wl[threadIdx.x] = g.w_low;
+      s_lh[threadIdx.x] = g.lh; s_lw[threadIdx.x] = g.lw;
+      s_pw[threadIdx.x] = pw[base + i];
+    }
+    __syncthreads();
+    const int n = min(256, n_pts - c0);
+    for (int j = 0; j < n; ++j) {
+      const int dh = py - s_hl[j], dw = px - s_wl[j];
+      if ((unsigned)dh <= 1u && (unsigned)dw <= 1u) {
+        const float wh = dh ? s_lh[j] : msda_sub(1.f, s_lh[j]);
+        const float ww = dw ? s_lw[j] : msda_sub(1.f, s_lw[j]);
+        a = msda_add(a, msda_mul(s_pw[j], msda_mul(wh, ww)));
+      }
+    }
+  }
+  if (p < H * W) density[((long long)l * R + r) * H * W + p] = a;
+}
+
+// d_map [R, HW, C] = sum over levels l in order of a[l, r, pixel] * (g[l, r, c] / cnt[l, r]), fp32, one bf16 rounding;
+// a level whose count is 0 adds nothing (the forward's 0 / 0 is zeroed by nan_to_num).  8 channels per thread.
+__global__ void __launch_bounds__(256)
+point_pool_outer_kernel(const float* __restrict__ density, const float* __restrict__ cnt, const __nv_bfloat16* __restrict__ grad,
+                        int L, int R, long long HW, int C, __nv_bfloat16* __restrict__ out) {
+  const int nvec = C / 8;
+  const long long total = (long long)R * HW * nvec;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(i % nvec);
+    const long long rp = i / nvec;                            // r * HW + pixel
+    const int r = (int)(rp / HW);
+    const long long p = rp - (long long)r * HW;
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+    for (int l = 0; l < L; ++l) {
+      const float c = cnt[(long long)l * R + r];
+      if (c == 0.f) continue;
+      const float a = density[((long long)l * R + r) * HW + p];
+      float g[8];
+      unpack8(__ldg(reinterpret_cast<const uint4*>(grad + ((long long)l * R + r) * C) + v), g);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = msda_add(acc[j], msda_mul(a, __fdiv_rn(g[j], c)));
+    }
+    *(reinterpret_cast<uint4*>(out + rp * C) + v) = pack8(acc);
+  }
+}
+
 // Segment sums of the assembly backward: positions sorted stably by destination row (dest[s], ascending, with order[s] the
 // position) -> every row r < n_rows of d_src = sum over the positions with destination r of dy[position], fp32 in
 // position order, one bf16 rounding; a row no position names is exact 0.  One CTA per destination row.
@@ -746,6 +902,79 @@ int vllm_layernorm_bwd_wb_bf16(const void* x, long long ldx, const void* dy, lon
     VLLM_CHECK_LAUNCH();
     return VLLM_OK;
   });
+}
+
+static int ln_gelu_bwd_rows_per_slot(long long rows) {
+  const long long target = (long long)vllm_num_sms() * 32;
+  return (int)((rows + target - 1) / target);
+}
+
+/* rows of dweight (and again of dbias) partials vllm_layernorm_gelu_bwd_bf16 needs for `rows` activation rows */
+long long vllm_layernorm_gelu_bwd_partials(long long rows) {
+  if (rows <= 0) return 0;
+  const int rps = ln_gelu_bwd_rows_per_slot(rows);
+  return (rows + rps - 1) / rps;
+}
+
+int vllm_layernorm_gelu_bwd_bf16(const void* x, long long ldx, const void* weight, const void* bias, const void* dy,
+                                 long long ldy, void* dx, long long lddx, float* dweight, float* dbias, float* partials,
+                                 long long n_partials, long long rows, int cols, float eps, void* stream) {
+  if (rows < 0 || cols <= 0) return VLLM_EINVAL;
+  if (cols % 8 || cols > 8 * 256 * 8) return VLLM_EUNSUPPORTED;
+  if (!dweight || !dbias) return VLLM_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rows == 0) {
+    const cudaError_t e = cudaMemsetAsync(dweight, 0, sizeof(float) * (size_t)cols, st);
+    return (int)(e != cudaSuccess ? e : cudaMemsetAsync(dbias, 0, sizeof(float) * (size_t)cols, st));
+  }
+  if (!x || !weight || !bias || !dy || !dx || !partials) return VLLM_EINVAL;
+  if (ldx % 8 || ldy % 8 || lddx % 8 || !vllm_aligned(x, 16) || !vllm_aligned(weight, 16) || !vllm_aligned(bias, 16) ||
+      !vllm_aligned(dy, 16) || !vllm_aligned(dx, 16) || !vllm_aligned(partials, 16))
+    return VLLM_EALIGN;
+  const int rps = ln_gelu_bwd_rows_per_slot(rows);
+  const long long slots = vllm_layernorm_gelu_bwd_partials(rows);
+  if (n_partials < slots) return VLLM_EINVAL;
+  auto go = [&](auto vpt, auto tpr) -> int {
+    constexpr int VPT = decltype(vpt)::value, TPR = decltype(tpr)::value;
+    const long long blocks = (slots + 256 / TPR - 1) / (256 / TPR);
+    layernorm_gelu_bwd_kernel<VPT, TPR><<<(unsigned)blocks, 256, 0, st>>>(
+        (const __nv_bfloat16*)x, ldx, (const __nv_bfloat16*)weight, (const __nv_bfloat16*)bias, (const __nv_bfloat16*)dy, ldy,
+        (__nv_bfloat16*)dx, lddx, rows, cols, eps, rps, slots, partials);
+    VLLM_CHECK_LAUNCH();
+    colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials, dweight, (int)slots, cols);
+    VLLM_CHECK_LAUNCH();
+    colsum_partials_kernel<<<(unsigned)((cols + 31) / 32), 256, 0, st>>>(partials + (size_t)slots * cols, dbias, (int)slots, cols);
+    VLLM_CHECK_LAUNCH();
+    return VLLM_OK;
+  };
+  // the forward's ladder (fused_ops.cu launch_norm): the statistics' reduction order, hence their bits, follow TPR
+  const int nvec = cols / 8;
+  if (nvec <= 128) return with_vpt<32, 1, 2, 4>(nvec, go);
+  if (nvec <= 1024) return with_vpt<128, 2, 4, 8>(nvec, go);
+  return with_vpt<256, 8>(nvec, go);
+}
+
+int vllm_point_pool_bwd_bf16(const float* loc, const float* weight, const float* counts, int n_points, const void* grad,
+                             int levels, int regions, int height, int width, int channels, float* density, void* d_map,
+                             void* stream) {
+  if (n_points < 0 || levels <= 0 || regions < 0 || height <= 0 || width <= 0 || channels <= 0) return VLLM_EINVAL;
+  if (channels % 8) return VLLM_EUNSUPPORTED;
+  if (regions == 0) return VLLM_OK;
+  if (!counts || !grad || !density || !d_map || (n_points > 0 && (!loc || !weight))) return VLLM_EINVAL;
+  if (!vllm_aligned(grad, 16) || !vllm_aligned(d_map, 16) || (n_points > 0 && !vllm_aligned(loc, 8))) return VLLM_EALIGN;
+  const long long HW = (long long)height * width;
+  if (HW > 2147483647LL || regions > 65535 || levels > 65535) return VLLM_EUNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  point_density_kernel<<<dim3((unsigned)((HW + 255) / 256), (unsigned)regions, (unsigned)levels), 256, 0, st>>>(
+      loc, weight, n_points, regions, height, width, density);
+  VLLM_CHECK_LAUNCH();
+  long long blocks = ((long long)regions * HW * (channels / 8) + 255) / 256;
+  const long long cap = (long long)vllm_num_sms() * 16;
+  if (blocks > cap) blocks = cap;
+  point_pool_outer_kernel<<<(unsigned)blocks, 256, 0, st>>>(density, counts, (const __nv_bfloat16*)grad, levels, regions, HW,
+                                                            channels, (__nv_bfloat16*)d_map);
+  VLLM_CHECK_LAUNCH();
+  return VLLM_OK;
 }
 
 int vllm_assemble_embeds_bwd_bf16(const int* dest, const int* order, long long n, const void* d_embeds, int hidden,

@@ -52,6 +52,26 @@ def rand_sample(x, divisor, max_len):
     return pts[:, indices].t()
 
 
+POOL_GROUP = 16                                  # points per MSDA query of the pooling
+
+
+def point_table(points, device):
+    """[region] -> [n_i, 3] (id, y, x in [0,1]) points -> the pooling's packed table: loc [B, n_pad, 2] fp32 (x, y) and
+    wgt [B, n_pad] fp32 (1 for a point, 0 for padding), n_pad the longest list rounded up to a query group of 16 (at
+    least one group).  The forward pools through it and the training backward transposes the same table."""
+    B, P = len(points), POOL_GROUP
+    n_max = max([len(p) for p in points] + [1])
+    Lq = (n_max + P - 1) // P
+    loc = torch.zeros(B, Lq * P, 2, dtype=torch.float32, device=device)
+    wgt = torch.zeros(B, Lq * P, dtype=torch.float32, device=device)
+    for i, p in enumerate(points):
+        n = len(p)
+        if n:
+            loc[i, :n] = p[:, -2:].flip(-1).float()                                         # (x, y)
+            wgt[i, :n] = 1.0
+    return loc, wgt
+
+
 def _patch_rows(x, k):
     """[B, H, W, C] channels-last -> [B*(H/k)*(W/k), C*k*k] rows in the (c, dy, dx) order of a Conv2d weight."""
     B, Hh, W, C = x.shape
@@ -112,22 +132,21 @@ class B200RegionEncoder(nn.Module):
         y = self._conv_rows(y, me[6], "c6")
         return y.view(B, h, w, -1)
 
-    def _pool_points(self, feat, points):
-        """feat [B, h, w, C]; points: list of [n_i, 3] (id, y, x in [0,1]) -> masked mean of the bilinear samples."""
+    def draw_points(self, masks, levels):
+        """The production draw: `rand_sample` per feature level and region, in the order the reference draws them
+        (:123-125) -> [level][region] -> [n, 3]."""
+        ori_h, ori_w = masks.shape[-2:]
+        divisor = torch.tensor([1, ori_h, ori_w], device=masks.device)[None,]
+        return [[rand_sample(m, divisor, self.num_points) for m in masks] for _ in range(levels)]
+
+    def _pool_points(self, feat, loc, wgt):
+        """feat [B, h, w, C]; the point table of `point_table` -> masked mean of the bilinear samples."""
         B, h, w, C = feat.shape
         D = 32
         if C % D:
             raise NotImplementedError("grid_sample pooling needs embed_dim % 32 == 0")
-        M, P = C // D, 16
-        n_max = max([len(p) for p in points] + [1])
-        Lq = (n_max + P - 1) // P
-        loc = torch.zeros(B, Lq * P, 2, dtype=torch.float32, device=feat.device)
-        wgt = torch.zeros(B, Lq * P, dtype=torch.float32, device=feat.device)
-        for i, p in enumerate(points):
-            n = len(p)
-            if n:
-                loc[i, :n] = p[:, -2:].flip(-1).float()                                     # (x, y)
-                wgt[i, :n] = 1.0
+        M, P = C // D, POOL_GROUP
+        Lq = loc.shape[1] // P
         shapes = msda_ext.attach_host_shapes(torch.tensor([[h, w]], dtype=torch.int64, device=feat.device), [(h, w)])
         lsi = torch.zeros(1, dtype=torch.int64, device=feat.device)
         value = feat.float().reshape(B, h * w, M, D).contiguous()
@@ -174,9 +193,7 @@ class B200RegionEncoder(nn.Module):
                 if sample_points is not None:
                     pts = sample_points[level]
                 else:                                   # a fresh draw per level, like the reference (:123-125)
-                    ori_h, ori_w = masks.shape[-2:]
-                    divisor = torch.tensor([1, ori_h, ori_w], device=masks.device)[None,]
-                    pts = [rand_sample(m, divisor, self.num_points) for m in masks]
-                out = self._pool_points(masks_out, pts)
+                    pts = self.draw_points(masks, 1)[0]
+                out = self._pool_points(masks_out, *point_table(pts, masks_out.device))
             outs.append(ops.linear(out.contiguous(), self.up_dim.weight, bias=self.up_dim.bias))
         return torch.stack(outs).mean(dim=0)

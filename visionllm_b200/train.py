@@ -116,6 +116,40 @@ def layernorm_bwd_wb(x2, dy2, eps):
     return dw, db
 
 
+def layernorm_gelu_bwd(x2, weight, bias, dy2, eps):
+    """Backward of ops.layernorm(..., gelu=True) on [rows, cols] bf16 rows: dx (bf16) and fp32 weight / bias gradients
+    summed in a fixed order (vllm_layernorm_gelu_bwd_bf16)."""
+    rows, cols = x2.shape
+    L = _lib.lib()
+    n_part = L.vllm_layernorm_gelu_bwd_partials(rows)
+    part = torch.empty((2 * max(n_part, 1), cols), dtype=torch.float32, device=x2.device)
+    dx = torch.empty_like(x2)
+    dw = torch.empty(cols, dtype=torch.float32, device=x2.device)
+    db = torch.empty(cols, dtype=torch.float32, device=x2.device)
+    with torch.cuda.device(x2.device):
+        rc = L.vllm_layernorm_gelu_bwd_bf16(x2.data_ptr(), x2.stride(0), weight.data_ptr(), bias.data_ptr(), dy2.data_ptr(),
+                                            dy2.stride(0), dx.data_ptr(), dx.stride(0), dw.data_ptr(), db.data_ptr(),
+                                            part.data_ptr(), n_part, rows, cols, float(eps), ops._stream())
+    _lib.check(rc, "vllm_layernorm_gelu_bwd_bf16")
+    return dx, dw, db
+
+
+def point_pool_bwd(loc, wgt, grad, h, w):
+    """Backward of the region encoder's point pooling over `levels` feature levels of one map: loc [levels, R, n, 2] /
+    wgt [levels, R, n] fp32 point tables (region_encoder.point_table, padded to one n), grad [levels, R, C] bf16 ->
+    d(map) [R, h * w, C] bf16 = sum_l a_l (x) grad_l / count_l (vllm_point_pool_bwd_bf16)."""
+    levels, R, n = wgt.shape
+    C = grad.shape[-1]
+    cnt = wgt.sum(2).contiguous()                                   # the forward's counts (wgt.sum(1) per level)
+    out = torch.empty((R, h * w, C), dtype=torch.bfloat16, device=grad.device)
+    density = torch.empty((levels, R, h * w), dtype=torch.float32, device=grad.device)
+    with torch.cuda.device(grad.device):
+        rc = _lib.lib().vllm_point_pool_bwd_bf16(loc.data_ptr(), wgt.data_ptr(), cnt.data_ptr(), n, grad.data_ptr(), levels, R,
+                                                 h, w, C, density.data_ptr(), out.data_ptr(), ops._stream())
+    _lib.check(rc, "vllm_point_pool_bwd_bf16")
+    return out
+
+
 def assemble_embeds_bwd(plan, d_embeds, source_rows, wanted):
     """Gradients of ops.assemble_embeds' sources from d(inputs_embeds) [B, L, C]: `source_rows` = rows of (token table, det
     table, pose table, image features), `wanted` = which of them need a gradient.  Positions are sorted stably by destination
@@ -607,6 +641,117 @@ class LayerNormWBFn(torch.autograd.Function):
         return None, dw.to(torch.bfloat16), db.to(torch.bfloat16), None
 
 
+class LayerNormGeluFn(torch.autograd.Function):
+    """LayerNorm over the last dim followed by exact-erf GELU (the region encoder's LayerNorm2d -> GELU on channels-last
+    rows), forward in one pass (ops.layernorm(gelu=True)), backward to the input, weight and bias in one pass."""
+
+    @staticmethod
+    def forward(ctx, x2, weight, bias, eps):
+        ctx.save_for_backward(x2, weight, bias)
+        ctx.eps = eps
+        return ops.layernorm(x2, weight, bias, eps, gelu=True)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x2, w, b = ctx.saved_tensors
+        dx, dw, db = layernorm_gelu_bwd(x2, w, b, dy.contiguous(), ctx.eps)
+        return dx, dw.to(w.dtype), db.to(b.dtype), None
+
+
+class RegionPoolFn(torch.autograd.Function):
+    """The region encoder's levels: masks_out accumulates each level's frozen features on the embedding (bf16 adds, in
+    level order) and every level pools it at its own points, exactly as B200RegionEncoder.forward.  Only the embedding takes
+    a gradient: d(emb) = sum over levels of the pooling's transpose (point_pool_bwd), one kernel pass for all levels.
+    emb [R, h, w, E]; feats: per level [R, h, w, E]; tables: per level (loc, wgt) of point_table.  -> [levels, R, E]."""
+
+    @staticmethod
+    def forward(ctx, emb, enc, feats, tables):
+        masks_out, pooled = emb, []
+        for f, (loc, wgt) in zip(feats, tables):
+            masks_out = masks_out + f.to(masks_out.dtype)
+            pooled.append(enc._pool_points(masks_out, loc, wgt))
+        n = max(t[1].shape[1] for t in tables)
+        loc = torch.stack([torch.nn.functional.pad(t[0], (0, 0, 0, n - t[0].shape[1])) for t in tables]).contiguous()
+        wgt = torch.stack([torch.nn.functional.pad(t[1], (0, n - t[1].shape[1])) for t in tables]).contiguous()
+        ctx.save_for_backward(loc, wgt)
+        ctx.hw = emb.shape[1:3]
+        return torch.stack(pooled)
+
+    @staticmethod
+    def backward(ctx, dpooled):
+        loc, wgt = ctx.saved_tensors
+        h, w = ctx.hw
+        d = point_pool_bwd(loc, wgt, dpooled.to(torch.bfloat16).contiguous(), h, w)
+        return d.view(d.shape[0], h, w, -1), None, None, None
+
+
+def _conv_weight(conv, k_pad):
+    """A Conv2d weight as the [Cout, Cin k k] GEMM operand (K zero-padded to k_pad), differentiable: its gradient lands on
+    the native [Cout, Cin, k, k] parameter."""
+    w = conv.weight.reshape(conv.out_channels, -1)
+    return torch.nn.functional.pad(w, (0, k_pad - w.shape[1])) if k_pad != w.shape[1] else w
+
+
+def region_encoder_train(enc, images, masks, image_features, sample_points=None):
+    """fwd of a 'grid_sample' B200RegionEncoder as autograd Functions on this repo's kernels, with gradients for every
+    parameter (mask_embedding.{0,1,3,4,6}, up_dim): the three convolutions are GEMMs over non-overlapping patches with the
+    bias in the epilogue (LinearFn), LayerNorm2d -> GELU is one row pass each way (LayerNormGeluFn), the k2s2 patch
+    rearrangement is a permute, the point pooling of every level is RegionPoolFn, up_dim one LinearFn per level, then the
+    mean over levels.  The forward values are B200RegionEncoder.forward's bytes for the same points.  sample_points:
+    [level][region] -> [n, 3] as the inference forward takes them; None draws them with rand_sample."""
+    from .region_encoder import _patch_rows, point_table
+    if enc.mask_pool_type != "grid_sample":
+        raise NotImplementedError(f"region-encoder training with mask_pool_type={enc.mask_pool_type!r}: only 'grid_sample' "
+                                  "(the reference's build_region_encoder builds no other)")
+    me = enc.mask_embedding
+    masks = masks.to(images.dtype)
+    x = torch.cat([images, masks], dim=1).permute(0, 2, 3, 1)                               # [B, H, W, 4]
+    B = x.shape[0]
+    rows, h, w = _patch_rows(x, me[0].kernel_size[0])
+    kp = (rows.shape[1] + 7) // 8 * 8
+    rows = torch.nn.functional.pad(rows, (0, kp - rows.shape[1])) if kp != rows.shape[1] else rows
+    y = LinearFn.apply(rows.contiguous(), _conv_weight(me[0], kp), False, None, me[0].bias)
+    y = LayerNormGeluFn.apply(y, me[1].weight, me[1].bias, me[1].eps)
+    rows, h, w = _patch_rows(y.view(B, h, w, -1), 2)
+    y = LinearFn.apply(rows.contiguous(), _conv_weight(me[3], rows.shape[1]), False, None, me[3].bias)
+    y = LayerNormGeluFn.apply(y, me[4].weight, me[4].bias, me[4].eps)
+    y = LinearFn.apply(y, _conv_weight(me[6], y.shape[1]), False, None, me[6].bias)
+    emb = y.view(B, h, w, -1)
+    feats = []
+    for f in image_features:
+        f = f.reshape(B, h, w, -1) if f.dim() == 3 else f.permute(0, 2, 3, 1)
+        assert f.shape[1:3] == (h, w)
+        feats.append(f)
+    pts = sample_points if sample_points is not None else enc.draw_points(masks, len(feats))
+    tables = [point_table(p, emb.device) for p in pts[:len(feats)]]
+    pooled = RegionPoolFn.apply(emb, enc, feats, tables)                                   # [levels, R, E]
+    outs = [LinearFn.apply(pooled[l], enc.up_dim.weight, False, None, enc.up_dim.bias) for l in range(len(feats))]
+    return torch.stack(outs).mean(dim=0)
+
+
+class RegionScatterFn(torch.autograd.Function):
+    """scatter_region_tokens with gradients: the forward writes the region features into the <region> rows; the backward
+    gathers d(embeds) at those rows for the features (vllm_gather_rows_bf16) and zeroes them for the assembly -- the
+    reference's inputs_embeds * (1 - region_mask) + features * region_mask, so no token-table row takes a gradient from a
+    <region> position."""
+
+    @staticmethod
+    def forward(ctx, embeds, feats, input_ids, reg_token_id):
+        from .modeling import scatter_region_tokens
+        rows = torch.nonzero((input_ids == reg_token_id).reshape(-1)).reshape(-1)
+        ctx.save_for_backward(rows)
+        return scatter_region_tokens(input_ids, embeds, feats, reg_token_id)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (rows,) = ctx.saved_tensors
+        B, L, C = dy.shape
+        d = dy.clone(memory_format=torch.contiguous_format).view(B * L, C)         # one copy: dy itself stays as it is
+        dfeat = ops.gather_rows(d, rows) if ctx.needs_input_grad[1] else None
+        d[rows] = 0
+        return d.view(B, L, C), dfeat, None, None
+
+
 class AssembleEmbedsFn(torch.autograd.Function):
     """ops.assemble_embeds with gradients for the token table, the two [EMB] tables and the image features."""
 
@@ -667,8 +812,12 @@ class B200VisionLLMv2ModelTrain(nn.Module):
     a `B200VisionLLMv2Model` (shared, not copied): the frozen vision encoder under no_grad, the vl_bridge, the sequence
     assembly (token table, [EMB] tables, image features) and the LLM decoder with gradients, on right-padded batches.
     Modules frozen with the composite's freeze_* methods get no gradient and cost no weight-gradient GEMM.
-    Refused (NotImplementedError): a trainable vision encoder, atom-tool losses (`targets`, `images_aug`), region-encoder
-    training (`regions`), the [EMB] insert form, KV caches, caller-provided `inputs_embeds`, non-CUDA / non-bf16 batches."""
+    With `regions`, the region encoder runs on the frozen ViT's last three hidden states (region_encoder_train, or its
+    inference forward after freeze_region_encoder()) and its features overwrite the <region> rows (RegionScatterFn);
+    `region_sample_points` ([level][region] -> [n, 3]) replaces the random point draw, as in the inference forward.
+    Refused (NotImplementedError): a trainable vision encoder, atom-tool losses (`targets`, `images_aug`), `regions` without
+    a region encoder or with a pooling other than 'grid_sample', the [EMB] insert form, KV caches, caller-provided
+    `inputs_embeds`, non-CUDA / non-bf16 batches."""
 
     def __init__(self, model):
         super().__init__()
@@ -679,7 +828,8 @@ class B200VisionLLMv2ModelTrain(nn.Module):
 
     def forward(self, input_ids=None, inputs_embeds=None, attention_mask=None, images=None, images_aug=None, img_metas=None,
                 targets=None, labels=None, past_key_values=None, use_cache=False, output_attentions=False,
-                output_hidden_states=False, return_dict=True, regions=None, num_splits=None, **unused):
+                output_hidden_states=False, return_dict=True, regions=None, num_splits=None, region_sample_points=None,
+                **unused):
         from .modeling import IGNORE_INDEX, VisionLLMv2ModelOutput
         m = self.model
         if past_key_values is not None or use_cache:
@@ -687,7 +837,11 @@ class B200VisionLLMv2ModelTrain(nn.Module):
         if targets is not None or images_aug is not None:
             raise NotImplementedError("atom-tool losses (detection / pose / generation targets) have no training path")
         if regions is not None:
-            raise NotImplementedError("region-encoder training has no training path")
+            if not getattr(m, "use_region_encoder", False):
+                raise NotImplementedError("regions on a composite built without a region encoder")
+            if m.region_encoder.mask_pool_type != "grid_sample":
+                raise NotImplementedError("region-encoder training pools with 'grid_sample' only (the reference's "
+                                          "build_region_encoder)")
         if inputs_embeds is not None or input_ids is None:
             raise NotImplementedError("the training step takes input_ids (the reference's collator batch)")
         _require_cuda_bf16(input_ids, m.llm.get_input_embeddings().weight,
@@ -697,7 +851,7 @@ class B200VisionLLMv2ModelTrain(nn.Module):
             if any(p.requires_grad for p in m.vis_encoder.parameters()):
                 raise NotImplementedError("a trainable vision encoder: call freeze_vis_encoder() (the reference's default)")
             with torch.no_grad():
-                hs, split_sizes, _ = m.vision_hidden_state(images)
+                hs, split_sizes, vit_out = m.vision_hidden_state(images)
             feats = bridge_train(m.vl_bridge, _bridge_input(m, hs))
         tokens_per_tile = 0
         if feats is not None:
@@ -715,6 +869,15 @@ class B200VisionLLMv2ModelTrain(nn.Module):
         pad = table.padding_idx if table.padding_idx is not None else getattr(m.llm.config, "pad_token_id", None)
         embeds = AssembleEmbedsFn.apply(plan, table.weight, m.emb_embeddings_det.weight, m.emb_embeddings_pose.weight, feats,
                                         pad if pad is not None and 0 <= pad < table.weight.shape[0] else None)
+        if regions is not None and images is not None:                                       # mv2.py:607-698
+            from .modeling import region_encoder_inputs
+            ri, rm, rf = region_encoder_inputs(images, regions, vit_out.hidden_states, split_sizes, num_splits)
+            enc = m.region_encoder
+            if any(p.requires_grad for p in enc.parameters()):
+                rfeat = region_encoder_train(enc, ri, rm, rf, region_sample_points)
+            else:                                                   # freeze_region_encoder(): the inference forward
+                rfeat = enc(ri, rm, rf, sample_points=region_sample_points)
+            embeds = RegionScatterFn.apply(embeds, rfeat, plan.new_ids, m.reg_token_id)
         if labels is not None:                                                               # mv2.py:740-757
             labels[(labels >= m.emb_token_id) & (labels <= m.emb_token_id + m.num_embs - 1)] = IGNORE_INDEX
         loss, logits, hidden = self.llm_train(embeds, labels=labels, attention_mask=attention_mask)
