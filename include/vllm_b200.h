@@ -448,7 +448,8 @@ int vllm_head_stack_bf16(const void* src, void* dst, int batch, int tokens, int 
  * then k heads, then v heads) -> Q [batch, nq, tokens, head_dim], K / V [batch, nkv, tokens, head_dim] (contiguous stacks
  * for vllm_gemm_bf16_batched_grouped) when to_stacked != 0, the inverse (stacked gradients -> packed d(qkv)) otherwise.
  * The pitch gap of a packed row is neither read nor written.  nq % nkv != 0 or ld < (nq + 2 nkv) head_dim: VLLM_EINVAL;
- * head_dim % 8: VLLM_EUNSUPPORTED; ld % 8 or a base not 16-byte aligned: VLLM_EALIGN. */
+ * head_dim % 8 (head_dim < 8 included; only batch * tokens == 0 returns VLLM_OK first): VLLM_EUNSUPPORTED; ld % 8 or a
+ * base not 16-byte aligned: VLLM_EALIGN. */
 int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void* v, int batch, int tokens, int nq, int nkv,
                              int head_dim, int to_stacked, void* stream);
 /* RMSNorm backward: dx bf16 and dweight fp32, the dweight reduction done through a workspace: every CTA writes its partial
@@ -473,6 +474,8 @@ int vllm_scale_rows_bf16(void* x, long long ld, long long rows, int cols, const 
  * rows per (batch, head) matrix (a multiple of 256 for the batched GEMMs).  vllm_head_stack_qkv_pad_bf16 is
  * vllm_head_stack_qkv_bf16 with stacks of tokens_pad rows: rows tokens .. tokens_pad - 1 are written as zeros going to the
  * stacks and are not read coming back; nkv = 0 stacks the nq heads of a plain [batch, tokens, nq head_dim] tensor (dO) into q.
+ * Rejections as vllm_head_stack_qkv_bf16 (head_dim < 8 is VLLM_EUNSUPPORTED, not a call that writes nothing), plus
+ * tokens_pad < tokens: VLLM_EINVAL.
  * vllm_softmax_causal_len_bf16 is vllm_softmax_causal_bf16 with key lengths lens[n_mat / heads_per_batch] (int32, device):
  * key j of query i is visible iff j <= i and j < lens[m / heads_per_batch]; P = 0 elsewhere (S is not used there), a row
  * with no visible key is all zeros.  n_mat % heads_per_batch: VLLM_EINVAL.  With lens == T it is bit-identical to

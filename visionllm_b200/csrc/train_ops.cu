@@ -690,10 +690,10 @@ int vllm_head_stack_qkv_bf16(void* packed, long long ld, void* q, void* k, void*
                              int head_dim, int to_stacked, void* stream) {
   if (batch < 0 || tokens < 0 || nq <= 0 || nkv <= 0 || head_dim <= 0 || nq % nkv) return VLLM_EINVAL;
   if (ld < (long long)(nq + 2 * nkv) * head_dim) return VLLM_EINVAL;
-  const long long n_vec = (long long)batch * tokens * (nq + 2 * nkv) * (head_dim / 8);
-  if (n_vec == 0) return VLLM_OK;
+  if ((long long)batch * tokens == 0) return VLLM_OK;
   if (!packed || !q || !k || !v) return VLLM_EINVAL;
-  if (head_dim % 8) return VLLM_EUNSUPPORTED;
+  if (head_dim % 8) return VLLM_EUNSUPPORTED;                 // before n_vec: head_dim < 8 would give no vectors at all
+  const long long n_vec = (long long)batch * tokens * (nq + 2 * nkv) * (head_dim / 8);
   if (ld % 8 || !vllm_aligned(packed, 16) || !vllm_aligned(q, 16) || !vllm_aligned(k, 16) || !vllm_aligned(v, 16))
     return VLLM_EALIGN;
   long long blocks = (n_vec + 255) / 256;
@@ -811,10 +811,10 @@ int vllm_head_stack_qkv_pad_bf16(void* packed, long long ld, void* q, void* k, v
   if (batch < 0 || tokens < 0 || tokens_pad < tokens || nq <= 0 || nkv < 0 || head_dim <= 0 || (nkv && nq % nkv))
     return VLLM_EINVAL;
   if (ld < (long long)(nq + 2 * nkv) * head_dim) return VLLM_EINVAL;
-  const long long n_vec = (long long)batch * tokens_pad * (nq + 2 * nkv) * (head_dim / 8);
-  if (n_vec == 0) return VLLM_OK;
+  if ((long long)batch * tokens_pad == 0) return VLLM_OK;
   if (!packed || !q || (nkv && (!k || !v))) return VLLM_EINVAL;
-  if (head_dim % 8) return VLLM_EUNSUPPORTED;
+  if (head_dim % 8) return VLLM_EUNSUPPORTED;                 // before n_vec: head_dim < 8 would give no vectors at all
+  const long long n_vec = (long long)batch * tokens_pad * (nq + 2 * nkv) * (head_dim / 8);
   if (ld % 8 || !vllm_aligned(packed, 16) || !vllm_aligned(q, 16) || !vllm_aligned(k, 16) || !vllm_aligned(v, 16))
     return VLLM_EALIGN;
   long long blocks = (n_vec + 255) / 256;
